@@ -2,6 +2,7 @@
 // every pair is two scalar FADD / FMUL / FFMA, each round-to-nearest, flush-to-zero, identical to the scalar instruction the
 // library's flags (--fmad=false -ftz=true) give.  The operations go through the _rn intrinsics, which ptxas never contracts
 // into an FFMA whatever feeds them.
+// tests/test_cpu_nlm_sass.py checks the built SASS: every FFMA of the NLM kernels is Markstein's division or part of an IEEE division.
 // With B200_KERNELS_ON_CPU (tests/emul) the same names are plain scalar code.
 #pragma once
 #ifdef B200_KERNELS_ON_CPU

@@ -177,3 +177,58 @@ extern "C" int emul_nlmeans_group(const float *in, float *out, int width, int he
     run_r<2>(g, n_ct * g.n_cl, norm1, profiled, divc);
   return g.G;
 }
+
+/* Which kernel, and which template instance of it, b200_nlmeans_denoise_dev launches for these arguments on a device offering smem_bytes of
+ * shared memory per block, and how many chunks take the pipelined kernel's half-height slots.  Only the host-side planning runs (the
+ * product's grp_define_patches, grp_plan, grp_pipe_fits, chunk_of, pipe2_takes); no kernel phase.  The development switches are read from the
+ * environment as the launcher reads them.  route[]: kernel (0 = nlm_chunks_kernel, 1 = nlm_chunks_win_kernel, 2 = nlm_pipe_kernel,
+ * 3 = nlm_group_kernel), R, WP, KP, N1, PR, DC, CFG, chunks on the half-height slots, chunks, patches in flight (group kernel). */
+extern "C" void emul_nlm_route(int width, int height, float scattering, float scale, float luma, float chroma, float center_weight, float sharpness,
+                               int radius, int search_radius, int decimate, const float *norm, int smem_bytes, int *route)
+{
+  for(int i = 0; i < 11; i++) route[i] = 0;
+  int n_patches = (2 * search_radius + 1) * (2 * search_radius + 1);
+  if(decimate) n_patches = (n_patches + 1) / 2;
+  std::vector<patch_t> patches(n_patches);
+  const int shift_max = grp_define_patches(patches.data(), search_radius, scale, scattering, decimate);
+  const float weight[4] = { luma, chroma, chroma, 1.0f }, invert[4] = { 1.0f - luma, 1.0f - chroma, 1.0f - chroma, 0.0f };
+  const int chk_h = slice_height(height), chk_w = slice_width(width);
+  const int n_chunks = ((height + chk_h - 1) / chk_h) * ((width + chk_w - 1) / chk_w);
+  route[9] = n_chunks;
+  route[1] = radius;
+  /* nlmeans_denoise_dev, nlm.cu:903-922 */
+  const bool chunks_forced = getenv("B200_NLM_CHUNKS") || getenv("B200_NLM_WINDOW");
+  grp_args_t g;
+  g.patches = patches.data();
+  int g_cap = GRP_MAXG;
+  if(const char *e = getenv("B200_NLM_G")) g_cap = atoi(e);
+  if(chunks_forced || !grp_plan(g, n_patches, width, height, radius, center_weight, sharpness, norm, weight, invert, (luma == 1.0 && chroma == 1.0) ? 1 : 0,
+                                shift_max, smem_bytes, g_cap))
+  {
+    const int rows_e = chk_h + 2 * radius + 1, cols_w = chk_w + 2 * radius + 2;
+    const long long win_bytes = 2LL * rows_e * cols_w * 16 + 2LL * chk_h * (cols_w | 1) * 4;
+    route[0] = getenv("B200_NLM_WINDOW") && win_bytes <= smem_bytes ? 1 : 0;
+    return;
+  }
+  /* launch_group, nlm.cu:795-824 (behind #ifndef B200_KERNELS_ON_CPU there, so restated here) */
+  const bool profiled = !(center_weight < 0), norm1 = norm[0] == 1.0f && norm[1] == 1.0f && norm[2] == 1.0f;
+  const bool divc = grp_division_by_constant(g) && !getenv("B200_NLM_IEEE_DIV");
+  route[4] = norm1;
+  route[5] = profiled;
+  route[6] = profiled && divc;
+  route[10] = g.G;
+  if(grp_pipe_fits(g, smem_bytes, pipe_cfg<0>::WP) && !getenv("B200_NLM_NO_PIPE"))
+  {
+    const int cfg = getenv("B200_NLM_WHOLE_SLOTS") ? 1 : 0;
+    route[0] = 2;
+    route[2] = cfg ? pipe_cfg<1>::WP : pipe_cfg<0>::WP;
+    route[3] = cfg ? pipe_cfg<1>::KP : pipe_cfg<0>::KP;
+    route[7] = cfg;
+    if(cfg == 0 && radius == 1) /* the kernel's own test, nlm_pipe_kernel in nlm_group.cuh */
+      for(int b = 0; b < n_chunks; b++) route[8] += pipe2_takes(g, chunk_of(g, b), radius) ? 1 : 0;
+    return;
+  }
+  route[0] = 3;
+  route[2] = g.wp;
+  route[3] = grp_pairs_per_thread(g) > GRP_KP_MIN ? GRP_KP_MAX : GRP_KP_MIN;
+}

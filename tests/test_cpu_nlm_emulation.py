@@ -3,15 +3,12 @@ thread, phase after phase, against the oracle bit for bit -- the packed fast pat
 division and the product's own host-side plan.  What it cannot see is nvcc's code generation (the `-m gpu` tests do).
 Test infrastructure only."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import util
 
-EMUL = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emul")
 SMEM = 232448  # cudaDevAttrMaxSharedMemoryPerBlockOptin of an H100 (227 KB)
 
 
@@ -21,12 +18,7 @@ def same_bits(a, b):
 
 @pytest.fixture(scope="module")
 def emul():
-    so = os.path.join(EMUL, "libemul_nlm.so")
-    csrc = os.path.join(util.ROOT, "ansel_b200", "csrc")
-    srcs = [os.path.join(EMUL, "emul_nlm.cpp"), os.path.join(EMUL, "cuda_on_cpu.h"), os.path.join(csrc, "nlm.cu"), os.path.join(csrc, "nlm_group.cuh")]
-    if not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fno-fast-math", "-ffp-contract=off", "-mfma", "-I", EMUL, "-shared", "-fPIC", "-o", so, srcs[0]], check=True)
-    return C.CDLL(so)
+    return util.emul_nlm()
 
 
 def emul_nlm(lib, img, *, scattering=0.0, scale=1.0, luma=1.0, chroma=1.0, center_weight=0.1, sharpness=0.005, P=1, K=7, decimate=0,

@@ -112,14 +112,6 @@ def test_nlmeans_full_width_strip_bit_exact(built, kw):
     assert not bad.any(), f"{int(bad.sum())} floats differ, first {np.argwhere(bad)[:4].tolist()}"
 
 
-def test_nlmeans_45mp_deterministic(built):
-    w, h = util.SIZE_45MP
-    img = (util.rgba_scene(w, h, util.SEEDS[2], noise=0.02) * 60).astype(np.float32)
-    a = cuda_nlm(img)
-    assert np.isfinite(a).all()
-    assert same_bits(a, cuda_nlm(img)).all()
-
-
 def test_chunk_kernel_is_bit_exact_too(built, monkeypatch):
     """the round-1 kernel (one chunk per CTA, patches one after the other): what runs where the group kernel's window does not fit"""
     monkeypatch.setenv("B200_NLM_CHUNKS", "1")
@@ -131,7 +123,9 @@ def test_chunk_kernel_is_bit_exact_too(built, monkeypatch):
 
 def test_extreme_pixels_through_the_group_kernel(built):
     """zeros (weights of exactly 1), infinities, NaN, values next to FLT_MAX and subnormals: Markstein's division, the clamp in
-    front of it and the packed lanes must leave what the reference leaves (tests/test_cpu_nlm_emulation.py has the same frame)"""
+    front of it and the packed lanes must leave what the reference leaves (tests/test_cpu_nlm_emulation.py has the same frame).
+    130 rows cut into chunks of 65: too tall for the pipelined kernel (64 rows at most), so this frame runs through the group kernel;
+    tests/test_zz_nlm_routes_gpu.py puts the same specials through the pipelined kernel's half-height slots"""
     img = (util.rgba_scene(160, 130, 4, noise=0.02) * 60).astype(np.float32)
     img[20:60, 30:90, :3] = 0.0
     img[70:90, 10:50, :3] = 1e-30

@@ -52,6 +52,39 @@ def ref(kind: str = "strict"):
     return _cache[key]
 
 
+def emul_nlm() -> C.CDLL:
+    """tests/emul/libemul_nlm.so: the non-local-means kernels' phases and the launcher's host-side plan compiled with g++
+    (rebuilt when a source is newer).  Test infrastructure, not part of the product."""
+    if "emul_nlm" not in _cache:
+        emul = os.path.join(ROOT, "tests", "emul")
+        so = os.path.join(emul, "libemul_nlm.so")
+        csrc = os.path.join(ROOT, "ansel_b200", "csrc")
+        srcs = [os.path.join(emul, "emul_nlm.cpp"), os.path.join(emul, "cuda_on_cpu.h"), os.path.join(csrc, "nlm.cu"),
+                os.path.join(csrc, "nlm_group.cuh"), os.path.join(csrc, "packed_f32.cuh")]
+        if not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs):
+            subprocess.run(["g++", "-O2", "-std=c++17", "-fno-fast-math", "-ffp-contract=off", "-mfma", "-I", emul, "-shared", "-fPIC", "-o", so,
+                            srcs[0]], check=True)
+        _cache["emul_nlm"] = C.CDLL(so)
+    return _cache["emul_nlm"]
+
+
+NLM_ROUTE_KERNELS = ("chunks", "window", "pipe", "group")
+
+
+def nlm_route(w, h, *, scattering=0.0, scale=1.0, luma=1.0, chroma=1.0, center_weight=0.1, sharpness=0.005, P=1, K=7, decimate=0,
+              norm=(1.0, 1.0, 1.0, 1.0), smem=232448):
+    """The kernel b200_nlmeans_denoise_dev launches for these arguments (the B200_NLM_* switches as the environment has them), predicted by
+    the product's own host-side planning: dict(kernel, R, WP, KP, N1, PR, DC, CFG, halves = chunks on the half-height slots, chunks,
+    G = patches in flight).  smem: shared memory per block an H100 opts into."""
+    r = (C.c_int * 11)()
+    emul_nlm().emul_nlm_route(w, h, C.c_float(scattering), C.c_float(scale), C.c_float(luma), C.c_float(chroma), C.c_float(center_weight),
+                              C.c_float(sharpness), P, K, decimate, (C.c_float * 4)(*norm), smem, r)
+    keys = ("kernel", "R", "WP", "KP", "N1", "PR", "DC", "CFG", "halves", "chunks", "G")
+    d = dict(zip(keys, list(r)))
+    d["kernel"] = NLM_ROUTE_KERNELS[d["kernel"]]
+    return d
+
+
 def fptr(a: np.ndarray):
     assert a.dtype == np.float32 and a.flags["C_CONTIGUOUS"]
     return a.ctypes.data_as(FP)
