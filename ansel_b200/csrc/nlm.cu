@@ -974,4 +974,14 @@ int denoiseprofile_nlmeans_dev(const b200_piece_t *piece, const b200_denoiseprof
   return B200_OK;
 }
 } // namespace b200
+
+#ifdef NLM_PIPE_TIMING
+// the device buffer nlm_pipe_kernel stores its per-warp role cycles in (PIPE_TIMING_WORDS per warp and block; nullptr: none)
+extern "C" int b200_nlm_pipe_timing(void *d_buf, int *words_per_warp)
+{
+  unsigned *p = (unsigned *)d_buf;
+  if(words_per_warp) *words_per_warp = PIPE_TIMING_WORDS;
+  return cudaMemcpyToSymbol(nlm_pipe_timing, &p, sizeof(p)) == cudaSuccess ? 0 : 1;
+}
+#endif
 #endif // B200_KERNELS_ON_CPU

@@ -375,14 +375,15 @@ __device__ __forceinline__ void grp_row_one(float *Sr /* Sr[col] = column sum of
   }
 }
 // two rows (lane x: row, lane y: row + half) of a patch with at least 2*R+1 columns; the column sum leaving the window
-// is the one read 2*R+1 steps earlier
-template <int R> __device__ __forceinline__ void grp_row_pair(float *Sx, float *Sy, const pgeo_t &g)
+// is the one read 2*R+1 steps earlier.  ZERO0: the column sum leaving at col_min is the column of zeros, taken as the constant
+// instead of read (x - 0 is x for every x, and no stored sum is subnormal)
+template <int R, bool ZERO0 = false> __device__ __forceinline__ void grp_row_pair(float *Sx, float *Sy, const pgeo_t &g)
 {
   constexpr int N = 2 * R + 1;
   float *px = Sx + g.col_min - R - 1, *py = Sy + g.col_min - R - 1; // slot of D[col_min], column sum leaving at col_min
   f2 ring[N];
   f2 distortion = mk2(0.0f, 0.0f);
-  ring[0] = mk2(px[0], py[0]);
+  ring[0] = ZERO0 ? mk2(0.0f, 0.0f) : mk2(px[0], py[0]);
 #pragma unroll
   for(int i = 1; i < N; i++)
   {
@@ -827,6 +828,11 @@ constexpr int PIPE_SCAN_GROUP = 128, PIPE_SLOTS = 3;
 // loads arrive in bursts in front of the scan warps' loads, and the scan warps are the critical path); phase B1 on two accumulating
 // warps (the scan groups then run phase A only, but the accumulators wait for a chain of 72 dependent steps every pair); 384
 // accumulating threads with 6 pairs each (64 registers for the scan threads spill their rings).
+// On H100 (45 MP bench frame, 400 W, tools/nlm_pipe_roles.py): no warp of the half-height path waits at a barrier for more than a few per
+// cent of the chunk -- every role works ~95 % of the time, and the phase-A walk sets the pace (removing its work moves the kernel time one
+// for one).  Measured slower there: the half walk fully unrolled (21 % fewer instructions, 20 % more kernel time: 36 KB more code for
+// the instruction caches next to the 19 KB accumulation loop); the two accumulating warps of a scheduler on the same half, in step
+// (4 % slower than staggered); IL = 3 on top of the unrolled walk (no change).
 template <int CFG> struct pipe_cfg
 {
   static constexpr int ACC_T = 256, KP = 9, L = 8, WP = 97, SCAN_REGS = 80, ACC_REGS = 176, NT = 2 * PIPE_SCAN_GROUP + ACC_T; // 256 x 80 + 256 x 176 = the register file
@@ -871,6 +877,10 @@ template <int R> __device__ __forceinline__ void pipe_b1(const grp_args_t &a, co
 // the scan warps that want the slot wait), HANDOVER[group] (scan warps and warp 3 meet: the half is written, and warp 3 is done with the
 // one before).  A slot is filled by the two groups in turn, three pairs apart; the group that fills it next reaches EMPTY[slot] only after it
 // has written a half that needed the other group's previous half consumed, i.e. long after the other group passed the same barrier.
+// Column 0 of a slot (the column of zeros) is never stored: phase B1 takes that column sum as the constant 0 (grp_row_pair<R, true>), so
+// warp 0 of a scan group no longer writes 64 zeros per half in a branch of its own.  The walk runs six rows per loop trip: with three,
+// the ring of squares and the prefetched row changed registers every trip and cost ~8 MOVs per row (44 instead of 36 instructions).
+// Measured on an H100 80GB HBM3 at 400 W, bench frame: nlm_pipe_kernel 33.4 -> 31.8 ms (column of zeros) -> 30.4 ms (six rows per trip).
 constexpr int PIPE2_SLOTS = 6, PIPE2_HROWS = 32, PIPE2_HSP = PIPE2_HROWS * GRP_SP; // floats of a half plane
 constexpr int PIPE2_A_T = 96, PIPE2_ACC_HALF = 128;
 constexpr int PIPE2_BAR_FULL = 1, PIPE2_BAR_EMPTY = PIPE2_BAR_FULL + PIPE2_SLOTS, PIPE2_BAR_HANDOVER = PIPE2_BAR_EMPTY + PIPE2_SLOTS; // 1..6, 7..12, 13..14
@@ -942,6 +952,7 @@ template <int WP, int R, bool NORM1> struct grp_colwalk_t
       step<2>(a, spa + GRP_SP, spb + GRP_SP);
       r = 2;
     }
+#pragma unroll 2 // six rows per trip: the registers of the ring and of the prefetched row come back where they started (no MOVs)
     for(; r + 3 <= PIPE2_HROWS; r += 3)
     {
       step<0>(a, spa + r * GRP_SP, spb + r * GRP_SP);
@@ -963,12 +974,54 @@ template <int R> __device__ __forceinline__ void pipe2_b1(const grp_args_t &a, c
   pgeo_t g;
   g.col_min = c.left;
   g.col_max = c.right;
-  grp_row_pair<R>(Sx, Sy, g);
+  grp_row_pair<R, true>(Sx, Sy, g); // column 0 of a half slot is never written: it holds the distortions of the half before
 }
 
 #ifndef B200_KERNELS_ON_CPU
 __device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 __device__ __forceinline__ void named_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+// ---- where the warps of nlm_pipe_kernel spend their cycles (development builds with -DNLM_PIPE_TIMING only) ----------------------
+// Every warp adds the clock() cycles between two marks to the role the interval belongs to; at its end lane 0 stores them, with the
+// warp's first and last clock and the path the chunk took, at words [(block * warps + warp) * PIPE_TIMING_WORDS ..] of the buffer
+// b200_nlm_pipe_timing() registered (tools/nlm_pipe_roles.py).  The product build compiles every mark to nothing.
+enum pipe_role_t { PIPE_ROLE_FILL, PIPE_ROLE_WORK, PIPE_ROLE_FULL, PIPE_ROLE_EMPTY, PIPE_ROLE_HANDOVER, PIPE_ROLE_GROUP, PIPE_ROLE_FINISH, PIPE_ROLES };
+constexpr int PIPE_TIMING_WORDS = PIPE_ROLES + 3; // + first clock, last clock, path (1: half-height slots, 2: whole-pair slots)
+#ifdef NLM_PIPE_TIMING
+__device__ unsigned *nlm_pipe_timing;
+struct pipe_clock_t
+{
+  unsigned t0, t, acc[PIPE_ROLES];
+  __device__ __forceinline__ pipe_clock_t()
+  {
+    t0 = t = (unsigned)clock();
+#pragma unroll
+    for(int r = 0; r < PIPE_ROLES; r++) acc[r] = 0u;
+  }
+  __device__ __forceinline__ void mark(int role)
+  {
+    const unsigned n = (unsigned)clock();
+    acc[role] += n - t;
+    t = n;
+  }
+  __device__ __forceinline__ void store(int path)
+  {
+    if(!nlm_pipe_timing || (threadIdx.x & 31)) return;
+    unsigned *const o = nlm_pipe_timing + ((size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * PIPE_TIMING_WORDS;
+#pragma unroll
+    for(int r = 0; r < PIPE_ROLES; r++) o[r] = acc[r];
+    o[PIPE_ROLES] = t0;
+    o[PIPE_ROLES + 1] = t;
+    o[PIPE_ROLES + 2] = path;
+  }
+};
+#else
+struct pipe_clock_t
+{
+  __device__ __forceinline__ void mark(int) {}
+  __device__ __forceinline__ void store(int) {}
+};
+#endif
 
 template <int R, bool NORM1, bool PROFILED, bool DIVC, int CFG>
 __global__ void __launch_bounds__(pipe_cfg<CFG>::NT, 1) nlm_pipe_kernel(const __grid_constant__ grp_args_t a)
@@ -979,10 +1032,12 @@ __global__ void __launch_bounds__(pipe_cfg<CFG>::NT, 1) nlm_pipe_kernel(const __
   float *const W = smem, *const S = smem + a.wrows * (3 * WP);
   int *const shifts = reinterpret_cast<int *>(S + 2 * PIPE_SLOTS * a.splane); // window shift of every patch
   const int tid = threadIdx.x;
+  pipe_clock_t clk;
   const chunk_t c = chunk_of(a, blockIdx.x);
   grp_fill<WP, NT>(a, c, W, tid);
   for(int p = tid; p < a.n_patches; p += NT) shifts[p] = grp_shift<WP>(a, p);
   __syncthreads();
+  clk.mark(PIPE_ROLE_FILL);
   const int npairs = (a.n_patches + 1) / 2;
   if constexpr(cfg::HALVES && R == 1)
   if(pipe2_takes(a, c, R))
@@ -1003,7 +1058,9 @@ __global__ void __launch_bounds__(pipe_cfg<CFG>::NT, 1) nlm_pipe_kernel(const __
           {
             const int w = 2 * q + hh, slot = w % PIPE2_SLOTS;
             float *const Sa = S + slot * (2 * PIPE2_HSP) + t, *const Sb = Sa + PIPE2_HSP;
+            clk.mark(PIPE_ROLE_WORK);
             if(w >= PIPE2_SLOTS) named_sync(PIPE2_BAR_EMPTY + slot, PIPE2_A_T + PIPE2_ACC_HALF);
+            clk.mark(PIPE_ROLE_EMPTY);
             if(live)
             {
               if(hh == 0)
@@ -1011,9 +1068,9 @@ __global__ void __launch_bounds__(pipe_cfg<CFG>::NT, 1) nlm_pipe_kernel(const __
               else
                 walk.template half<(PIPE2_HROWS % 3)>(a, Sa, Sb);
             }
-            else if(t == 0)
-              for(int rr = 0; rr < PIPE2_HROWS; rr++) Sa[rr * GRP_SP] = Sb[rr * GRP_SP] = 0.0f; // the column of zeros left of the first live one (:228-231)
+            clk.mark(PIPE_ROLE_WORK);
             named_sync(PIPE2_BAR_HANDOVER + group, PIPE_SCAN_GROUP);
+            clk.mark(PIPE_ROLE_HANDOVER);
           }
         }
       }
@@ -1024,11 +1081,15 @@ __global__ void __launch_bounds__(pipe_cfg<CFG>::NT, 1) nlm_pipe_kernel(const __
           for(int hh = 0; hh < 2; hh++)
           {
             const int slot = (2 * q + hh) % PIPE2_SLOTS;
+            clk.mark(PIPE_ROLE_WORK);
             named_sync(PIPE2_BAR_HANDOVER + group, PIPE_SCAN_GROUP);
+            clk.mark(PIPE_ROLE_HANDOVER);
             pipe2_b1<R>(a, c, S + slot * (2 * PIPE2_HSP), 2 * q, l);
             named_arrive(PIPE2_BAR_FULL + slot, 32 + PIPE2_ACC_HALF);
           }
       }
+      clk.mark(PIPE_ROLE_WORK);
+      clk.store(1);
     }
     else
     {
@@ -1041,12 +1102,17 @@ __global__ void __launch_bounds__(pipe_cfg<CFG>::NT, 1) nlm_pipe_kernel(const __
       {
         const int w = 2 * q + hh, slot = w % PIPE2_SLOTS;
         const float *const Sa = S + slot * (2 * PIPE2_HSP);
+        clk.mark(PIPE_ROLE_WORK);
         named_sync(PIPE2_BAR_FULL + slot, 32 + PIPE2_ACC_HALF);
+        clk.mark(PIPE_ROLE_FULL);
         grp_accumulate_pairs<WP, PROFILED, DIVC>(a, W + shifts[2 * q], Sa, st);
         if(2 * q + 1 < a.n_patches) grp_accumulate_pairs<WP, PROFILED, DIVC>(a, W + shifts[2 * q + 1], Sa + PIPE2_HSP, st);
         if(w + PIPE2_SLOTS < 2 * npairs) named_arrive(PIPE2_BAR_EMPTY + slot, PIPE2_A_T + PIPE2_ACC_HALF);
       }
+      clk.mark(PIPE_ROLE_WORK);
       grp_finish(a, c, st, ta, hh * PIPE2_HROWS);
+      clk.mark(PIPE_ROLE_FINISH);
+      clk.store(1);
     }
     return;
   }
@@ -1060,12 +1126,18 @@ __global__ void __launch_bounds__(pipe_cfg<CFG>::NT, 1) nlm_pipe_kernel(const __
     {
       const int slot = q % PIPE_SLOTS;
       float *const Sa = S + (2 * slot) * a.splane, *const Sb = Sa + a.splane;
+      clk.mark(PIPE_ROLE_WORK);
       if(q >= PIPE_SLOTS) named_sync(PIPE_BAR_EMPTY + slot, PIPE_SCAN_GROUP + ACC_T);
+      clk.mark(PIPE_ROLE_EMPTY);
       if(t < c.ncols) grp_scan_column<WP, R, NORM1>(a, c, W, Sa, Sb, 2 * q, t);
+      clk.mark(PIPE_ROLE_WORK);
       named_sync(PIPE_BAR_GROUP + group, PIPE_SCAN_GROUP);
+      clk.mark(PIPE_ROLE_GROUP);
       pipe_b1<R>(a, c, Sa, 2 * q, tb, half);
       named_arrive(PIPE_BAR_FULL + slot, PIPE_SCAN_GROUP + ACC_T);
     }
+    clk.mark(PIPE_ROLE_WORK);
+    clk.store(2);
   }
   else
   {
@@ -1081,7 +1153,9 @@ __global__ void __launch_bounds__(pipe_cfg<CFG>::NT, 1) nlm_pipe_kernel(const __
       {
         const int slot = q % PIPE_SLOTS;
         const float *const Sa = S + (2 * slot) * a.splane;
+        clk.mark(PIPE_ROLE_WORK);
         named_sync(PIPE_BAR_FULL + slot, PIPE_SCAN_GROUP + ACC_T);
+        clk.mark(PIPE_ROLE_FULL);
         grp_accumulate_pairs<WP, PROFILED, DIVC>(a, W + shifts[2 * q], Sa, st);
         if(2 * q + 1 < a.n_patches) grp_accumulate_pairs<WP, PROFILED, DIVC>(a, W + shifts[2 * q + 1], Sa + a.splane, st);
         if(q + PIPE_SLOTS < npairs) named_arrive(PIPE_BAR_EMPTY + slot, PIPE_SCAN_GROUP + ACC_T);
@@ -1093,13 +1167,18 @@ __global__ void __launch_bounds__(pipe_cfg<CFG>::NT, 1) nlm_pipe_kernel(const __
       {
         const int slot = q % PIPE_SLOTS;
         const float *const Sa = S + (2 * slot) * a.splane;
+        clk.mark(PIPE_ROLE_WORK);
         named_sync(PIPE_BAR_FULL + slot, PIPE_SCAN_GROUP + ACC_T);
+        clk.mark(PIPE_ROLE_FULL);
         grp_accumulate_edge<WP, PROFILED, DIVC>(a, c, W, Sa, st, 2 * q);
         grp_accumulate_edge<WP, PROFILED, DIVC>(a, c, W, Sa + a.splane, st, 2 * q + 1);
         if(q + PIPE_SLOTS < npairs) named_arrive(PIPE_BAR_EMPTY + slot, PIPE_SCAN_GROUP + ACC_T);
       }
     }
+    clk.mark(PIPE_ROLE_WORK);
     grp_finish(a, c, st, ta);
+    clk.mark(PIPE_ROLE_FINISH);
+    clk.store(2);
   }
 }
 #endif
