@@ -833,6 +833,14 @@ constexpr int PIPE_SCAN_GROUP = 128, PIPE_SLOTS = 3;
 // for one).  Measured slower there: the half walk fully unrolled (21 % fewer instructions, 20 % more kernel time: 36 KB more code for
 // the instruction caches next to the 19 KB accumulation loop); the two accumulating warps of a scheduler on the same half, in step
 // (4 % slower than staggered); IL = 3 on top of the unrolled walk (no change).
+// Pitches of the half-height path's 64-bit layout (pipe2_fill), WP = 97 and slot rows of GRP_SP = 77 f2, both odd.  A 64-bit access is
+// served per half-warp: conflict-free when its 16 double-words fall in 16 distinct bank pairs (word index mod 16).  Phase A (lanes =
+// consecutive columns of one row) and the fill are conflict-free at any pitch.  Phase B1 (lanes = the 32 rows of a half, one column):
+// rows differ by 77 f2 -> an odd pitch.  Phase B2 (L = 8 strips: 8 consecutive columns on rows 8 apart per half-warp; four such groups per
+// warp for c2): 8 * 77 = 8 (mod 16) for the slots, 8 * 97 = 8 (mod 16) for the f2 window plane, 8 * 97 = 8 (mod 32) for the c2 plane.
+// A uniform patch shift moves every lane by the same offset and changes nothing.  Which is why the window is two planes and not rows
+// of an f2 line followed by a c2 line: an f2 line needs an even row pitch (3 * WP even), and then rows 8 apart sit 0 or 16 banks apart,
+// a two-way conflict on every c2 load of phase B2.  tools/nlm_pipe_banks.py checks every access at every shift of K = 7.
 template <int CFG> struct pipe_cfg
 {
   static constexpr int ACC_T = 256, KP = 9, L = 8, WP = 97, SCAN_REGS = 80, ACC_REGS = 176, NT = 2 * PIPE_SCAN_GROUP + ACC_T; // 256 x 80 + 256 x 176 = the register file
@@ -881,6 +889,10 @@ template <int R> __device__ __forceinline__ void pipe_b1(const grp_args_t &a, co
 // warp 0 of a scan group no longer writes 64 zeros per half in a branch of its own.  The walk runs six rows per loop trip: with three,
 // the ring of squares and the prefetched row changed registers every trip and cost ~8 MOVs per row (44 instead of 36 instructions).
 // Measured on an H100 80GB HBM3 at 400 W, bench frame: nlm_pipe_kernel 33.4 -> 31.8 ms (column of zeros) -> 30.4 ms (six rows per trip).
+// These chunks keep the window and the slots in a layout of their own (pipe2_fill, pipe_cfg): a thread's two neighbouring values are one
+// 64-bit access, which halves the shared-memory instructions at the same number of wavefronts; the helpers above (grp_colwalk_t, pipe2_b1)
+// are those of the plain layout, which the group kernel and the emulation of the plain layout use.  Measured on an H100 80GB HBM3 at 700 W,
+// bench frame, three alternated runs per build: nlm_pipe_kernel 26.9 -> 25.9 ms (phase-A loop 42.5 -> 39 instructions per row).
 constexpr int PIPE2_SLOTS = 6, PIPE2_HROWS = 32, PIPE2_HSP = PIPE2_HROWS * GRP_SP; // floats of a half plane
 constexpr int PIPE2_A_T = 96, PIPE2_ACC_HALF = 128;
 constexpr int PIPE2_BAR_FULL = 1, PIPE2_BAR_EMPTY = PIPE2_BAR_FULL + PIPE2_SLOTS, PIPE2_BAR_HANDOVER = PIPE2_BAR_EMPTY + PIPE2_SLOTS; // 1..6, 7..12, 13..14
@@ -977,6 +989,282 @@ template <int R> __device__ __forceinline__ void pipe2_b1(const grp_args_t &a, c
   grp_row_pair<R, true>(Sx, Sy, g); // column 0 of a half slot is never written: it holds the distortions of the half before
 }
 
+// ---- the half-height path's shared-memory layout: 64-bit accesses where a thread reads or writes two neighbouring values ----------
+// Window: two planes of WP-element rows, one of float2 {c0, c1} and one of c2 (3 * WP floats per row, as grp_fill's); element (r, c)
+// sits at r * WP + c in both, so a patch shift is one element offset for both planes.  Slots: one plane per half of a patch pair
+// that holds f2 {patch a, patch b} per (row, column), rows of GRP_SP f2 (the two planes of the same slot, interleaved).  Bank
+// reasoning at pipe_cfg; tools/nlm_pipe_banks.py checks it.
+__device__ __forceinline__ float *pipe2_w2(float *W, int wrows, int wp) { return W + 2 * wrows * wp; } // the c2 plane behind the f2 plane
+// the first float of the slots, rounded up to 8 bytes (2 * PIPE2_SLOTS * PIPE2_HSP + 1 floats fit the room of the whole-pair slots)
+__device__ __forceinline__ f2 *pipe2_slots(float *smem, int wrows, int wp) { return reinterpret_cast<f2 *>(smem + ((wrows * 3 * wp + 1) & ~1)); }
+static_assert(2 * PIPE2_SLOTS * PIPE2_HSP + 1 <= 2 * PIPE_SLOTS * (2 * PIPE2_HROWS + 1) * GRP_SP, "the aligned half slots fit the room of the whole-pair slots");
+
+template <int WP, int NTHREADS> __device__ __forceinline__ void pipe2_fill(const grp_args_t &a, const chunk_t &c, float *W, int tid)
+{
+  f2 *const W01 = reinterpret_cast<f2 *>(W);
+  float *const W2 = pipe2_w2(W, a.wrows, WP);
+  const int n = a.wrows * a.wcols;
+  for(int idx = tid; idx < n; idx += NTHREADS)
+  {
+    const int wi = idx / a.wcols, wj = idx - wi * a.wcols;
+    const int r = c.wr0 + wi, col = c.wc0 + wj;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if(r >= 0 && r < a.height && col >= 0 && col < a.width) v = __ldg(a.in + (size_t)r * a.width + col);
+    W01[wi * WP + wj] = mk2(v.x, v.y);
+    W2[wi * WP + wj] = v.z;
+  }
+}
+template <int WP> __device__ __forceinline__ int pipe2_shift(const grp_args_t &a, int p) { return a.patches[p].rows * WP + a.patches[p].cols; }
+
+// phase A of two patches down one column (grp_colwalk_t on the paired window): a row is three LDS.64 and three LDS.32, its sums one STS.64
+template <int WP, bool NORM1> struct pipe2_colwalk_t
+{
+  static constexpr int N = 3;
+  f2 ring[N][3];
+  f2 cs;
+  f2 nx, na, nb; // the prefetched row: {c0, c1} of the pixel and of its two partners
+  float nx2, na2, nb2;
+  const f2 *x, *ya, *yb;
+  const float *x2, *ya2, *yb2;
+  __device__ __forceinline__ void load()
+  {
+    nx = x[0];
+    na = ya[0];
+    nb = yb[0];
+    nx2 = x2[0];
+    na2 = ya2[0];
+    nb2 = yb2[0];
+  }
+  __device__ __forceinline__ void advance()
+  {
+    x += WP;
+    ya += WP;
+    yb += WP;
+    x2 += WP;
+    ya2 += WP;
+    yb2 += WP;
+  }
+  __device__ __forceinline__ grp_row9_t row() const { return grp_row9_t{ nx.x, nx.y, nx2, na.x, na.y, na2, nb.x, nb.y, nb2 }; }
+  __device__ __forceinline__ void init(const grp_args_t &a, const chunk_t &c, const float *W, int pa, int k)
+  {
+    const int o = (c.top - 1 - c.wr0) * WP + (c.cbase + k - c.wc0);
+    const int pb = pa + 1 < a.n_patches ? pa + 1 : pa; // the last patch of an odd list walks alone: its twin is itself, its values unread
+    const int sa = a.patches[pa].rows * WP + a.patches[pa].cols, sb = a.patches[pb].rows * WP + a.patches[pb].cols;
+    const f2 *const W01 = reinterpret_cast<const f2 *>(W);
+    const float *const W2 = W + 2 * a.wrows * WP;
+    x = W01 + o;
+    ya = x + sa;
+    yb = x + sb;
+    x2 = W2 + o;
+    ya2 = x2 + sa;
+    yb2 = x2 + sb;
+    cs = mk2(0.0f, 0.0f);
+    load();
+#pragma unroll
+    for(int i = 0; i < N; i++)
+    {
+      const grp_row9_t cur = row();
+      advance();
+      load();
+      grp_squares2(cur, ring[i][0], ring[i][1], ring[i][2]);
+      cs = add2(cs, grp_pd2<NORM1>(ring[i][0], ring[i][1], ring[i][2], mk2(a.norm[0], a.norm[0]), mk2(a.norm[1], a.norm[1]), mk2(a.norm[2], a.norm[2])));
+    }
+  }
+  template <int S> __device__ __forceinline__ void step(const grp_args_t &a, f2 *sp)
+  {
+    const grp_row9_t cur = row();
+    advance();
+    load();
+    *sp = cs;
+    f2 e0, e1, e2;
+    grp_squares2(cur, e0, e1, e2);
+    cs = add2(cs, grp_pd2<NORM1>(sub2(e0, ring[S][0]), sub2(e1, ring[S][1]), sub2(e2, ring[S][2]), mk2(a.norm[0], a.norm[0]), mk2(a.norm[1], a.norm[1]),
+                                 mk2(a.norm[2], a.norm[2])));
+    ring[S][0] = e0;
+    ring[S][1] = e1;
+    ring[S][2] = e2;
+  }
+  // 32 rows of a half slot starting at ring place S0; sp: the thread's column in the slot's first row
+  template <int S0> __device__ __forceinline__ void half(const grp_args_t &a, f2 *sp)
+  {
+    int r = 0;
+    if(S0 == 2)
+    {
+      step<2>(a, sp);
+      r = 1;
+    }
+    else if(S0 == 1)
+    {
+      step<1>(a, sp);
+      step<2>(a, sp + GRP_SP);
+      r = 2;
+    }
+#pragma unroll 2 // six rows per trip, as grp_colwalk_t::half
+    for(; r + 3 <= PIPE2_HROWS; r += 3)
+    {
+      step<0>(a, sp + r * GRP_SP);
+      step<1>(a, sp + (r + 1) * GRP_SP);
+      step<2>(a, sp + (r + 2) * GRP_SP);
+    }
+    if(r < PIPE2_HROWS) step<0>(a, sp + r * GRP_SP), r++;
+    if(r < PIPE2_HROWS) step<1>(a, sp + r * GRP_SP);
+  }
+};
+
+// phase B1 of one half slot for lane l of the group's warp 3: row l of both patches (lane x: patch a, lane y: patch b), grp_row_pair<R, true>
+// on f2 column sums -- the same additions in the same order per (patch, row), one LDS.64 and one STS.64 per column
+template <int R> __device__ __forceinline__ void pipe2_b1_rows(const chunk_t &c, f2 *Sh, int l)
+{
+  constexpr int N = 2 * R + 1;
+  f2 *p = Sh + l * GRP_SP + (c.left - R - 1 - c.cbase); // slot of D[left], column sum leaving at left (column 0: never stored, taken as 0)
+  f2 ring[N];
+  f2 distortion = mk2(0.0f, 0.0f);
+  ring[0] = mk2(0.0f, 0.0f);
+#pragma unroll
+  for(int i = 1; i < N; i++)
+  {
+    ring[i] = p[i];
+    distortion = add2(distortion, ring[i]);
+  }
+  f2 nxt[N];
+#pragma unroll
+  for(int s = 0; s < N; s++) nxt[s] = p[s + N];
+  int left = c.right - c.left;
+  for(; left >= N; left -= N)
+  {
+    f2 cur[N];
+#pragma unroll
+    for(int s = 0; s < N; s++) cur[s] = nxt[s];
+#pragma unroll
+    for(int s = 0; s < N; s++) nxt[s] = p[s + 2 * N];
+#pragma unroll
+    for(int s = 0; s < N; s++)
+    {
+      distortion = add2(distortion, sub2(cur[s], ring[s]));
+      ring[s] = cur[s];
+      p[s] = distortion;
+    }
+    p += N;
+  }
+#pragma unroll
+  for(int s = 0; s < N; s++)
+  {
+    if(s < left)
+    {
+      distortion = add2(distortion, sub2(nxt[s], ring[s]));
+      p[s] = distortion;
+    }
+  }
+}
+
+// grp_own_init (strip ownership) on the paired window: wofs0 counts elements of a plane (r * WP + c), each pixel one LDS.64 + one LDS.32
+template <int WP, int KP, int L, int IL>
+__device__ __forceinline__ void pipe2_own_init(const grp_args_t &a, const chunk_t &c, const float *W, grp_strip_t<KP, L, IL> &st, int ta)
+{
+  int pr, i;
+  grp_strip_of<L>(ta, pr, i);
+  const bool rows = 2 * pr < c.ch;
+  const int r0 = rows ? 2 * pr : 0;
+  st.wofs0 = (c.top + r0 - c.wr0) * WP + (c.left + i - c.wc0);
+  st.sofs0 = r0 * GRP_SP + i;
+  st.lower = st.upper = 0u;
+  const f2 *const W01 = reinterpret_cast<const f2 *>(W);
+  const float *const W2 = W + 2 * a.wrows * WP;
+#pragma unroll
+  for(int k = 0; k < KP; k++)
+  {
+#pragma unroll
+    for(int j = 0; j < 8; j++) st.acc[k][j] = 0.0f;
+    if(rows && i + k * L < c.cw)
+    {
+      st.upper |= 1u << k;
+      if(2 * pr + 1 < c.ch) st.lower |= 1u << k;
+    }
+    const f2 u = W01[st.wofs(k)], d = W01[st.wofs(k) + WP];
+    st.ctr[k][0] = u.x;
+    st.ctr[k][1] = d.x;
+    st.ctr[k][2] = u.y;
+    st.ctr[k][3] = d.y;
+    st.ctr[k][4] = W2[st.wofs(k)];
+    st.ctr[k][5] = W2[st.wofs(k) + WP];
+  }
+}
+
+// one pixel pair (acc, ctr: its slots in the strip) and one patch: grp_accumulate_pairs' arithmetic for IL = 1, operation for operation
+template <bool PROFILED, bool DIVC>
+__device__ __forceinline__ void pipe2_weigh(const grp_args_t &a, f2 q0, f2 q1, f2 q2, f2 t, const float *ctr, float *acc)
+{
+  if(PROFILED)
+  { // :404-420
+    f2 e0 = sub2(mk2(ctr[0], ctr[1]), q0), e1 = sub2(mk2(ctr[2], ctr[3]), q1), e2 = sub2(mk2(ctr[4], ctr[5]), q2);
+    e0 = mul2(e0, e0);
+    e1 = mul2(e1, e1);
+    e2 = mul2(e2, e2);
+    const f2 cp = mk2(a.cp_norm, a.cp_norm);
+    e0 = mul2(e0, cp);
+    e1 = mul2(e1, cp);
+    e2 = mul2(e2, cp);
+    e0 = mk2(e0.x + e1.x, e0.y + e1.y);
+    e0 = mk2(e0.x + e2.x, e0.y + e2.y);
+    t = add2(t, e0);
+    if(DIVC)
+    { // x / d, correctly rounded (grp_accumulate_pairs)
+      const f2 ndd = mk2(-a.div_d, -a.div_d), rcp = mk2(a.div_rcp, a.div_rcp);
+      t = mk2(min_nan(t.x, 3.402823466e38f), min_nan(t.y, 3.402823466e38f));
+      e1 = mul2(t, rcp);
+      e2 = fma2(e1, ndd, t);
+      t = fma2(e2, rcp, e1);
+    }
+    else
+      t = mk2(t.x / a.div_d, t.y / a.div_d);
+    t = mul2(t, mk2(a.sharpness, a.sharpness));
+    t = mk2(t.x - 2.0f, t.y - 2.0f);
+    t = mk2(fmaxf(0.0f, t.x), fmaxf(0.0f, t.y));
+  }
+  else
+    t = mul2(t, mk2(a.sharpness, a.sharpness)); // :389-402
+  t = mk2(grp_mexp2_daz<!PROFILED>(t.x), grp_mexp2_daz<!PROFILED>(t.y)); // the weights
+  q0 = mk2(q0.x * t.x, q0.y * t.y); // out += pixel * wt: products per lane, sums packed
+  q1 = mk2(q1.x * t.x, q1.y * t.y);
+  q2 = mk2(q2.x * t.x, q2.y * t.y);
+  const f2 a0 = add2(mk2(acc[0], acc[1]), q0), a1 = add2(mk2(acc[2], acc[3]), q1), a2 = add2(mk2(acc[4], acc[5]), q2), a3 = add2(mk2(acc[6], acc[7]), t);
+  acc[0] = a0.x;
+  acc[1] = a0.y;
+  acc[2] = a1.x;
+  acc[3] = a1.y;
+  acc[4] = a2.x;
+  acc[5] = a2.y;
+  acc[6] = a3.x;
+  acc[7] = a3.y;
+}
+// phase B2 of one half slot: every pixel pair of the thread, patch a then (both: the pair has two patches) patch b.  Sh: the slot
+// ({a, b} per row and column), sa / sb: the patches' element shifts (pipe2_shift).  A pixel's two distortions are one LDS.64, its
+// partner's {c0, c1} one LDS.64 and c2 one LDS.32.  Every accumulator still takes patch a before patch b.
+template <int WP, bool PROFILED, bool DIVC, class ST>
+__device__ __forceinline__ void pipe2_accumulate(const grp_args_t &a, const float *W, const f2 *Sh, int sa, int sb, bool both, ST &st)
+{
+  constexpr int KP = ST::KP;
+  const f2 *const W01 = reinterpret_cast<const f2 *>(W);
+  const float *const W2 = W + 2 * a.wrows * WP;
+  const f2 *const Wa = W01 + sa, *const Wb = W01 + sb;
+  const float *const Wa2 = W2 + sa, *const Wb2 = W2 + sb;
+#pragma unroll
+  for(int k = 0; k < KP; k++)
+  {
+    const f2 du = Sh[st.sofs(k)], dl = Sh[st.sofs(k) + GRP_SP]; // {a, b} of the upper and of the lower pixel
+    const int o = st.wofs(k);
+    {
+      const f2 u = Wa[o], d = Wa[o + WP];
+      pipe2_weigh<PROFILED, DIVC>(a, mk2(u.x, d.x), mk2(u.y, d.y), mk2(Wa2[o], Wa2[o + WP]), mk2(du.x, dl.x), st.ctr[k], st.acc[k]);
+    }
+    if(both)
+    {
+      const f2 u = Wb[o], d = Wb[o + WP];
+      pipe2_weigh<PROFILED, DIVC>(a, mk2(u.x, d.x), mk2(u.y, d.y), mk2(Wb2[o], Wb2[o + WP]), mk2(du.y, dl.y), st.ctr[k], st.acc[k]);
+    }
+  }
+}
+
 #ifndef B200_KERNELS_ON_CPU
 __device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 __device__ __forceinline__ void named_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
@@ -1034,14 +1322,24 @@ __global__ void __launch_bounds__(pipe_cfg<CFG>::NT, 1) nlm_pipe_kernel(const __
   const int tid = threadIdx.x;
   pipe_clock_t clk;
   const chunk_t c = chunk_of(a, blockIdx.x);
-  grp_fill<WP, NT>(a, c, W, tid);
-  for(int p = tid; p < a.n_patches; p += NT) shifts[p] = grp_shift<WP>(a, p);
+  const bool halves = cfg::HALVES && R == 1 && pipe2_takes(a, c, R); // uniform over the block: it picks the window's layout
+  if(halves)
+  {
+    pipe2_fill<WP, NT>(a, c, W, tid);
+    for(int p = tid; p < a.n_patches; p += NT) shifts[p] = pipe2_shift<WP>(a, p);
+  }
+  else
+  {
+    grp_fill<WP, NT>(a, c, W, tid);
+    for(int p = tid; p < a.n_patches; p += NT) shifts[p] = grp_shift<WP>(a, p);
+  }
   __syncthreads();
   clk.mark(PIPE_ROLE_FILL);
   const int npairs = (a.n_patches + 1) / 2;
   if constexpr(cfg::HALVES && R == 1)
-  if(pipe2_takes(a, c, R))
-  { // ---- half-height slots (see PIPE2_SLOTS) ----
+  if(halves)
+  { // ---- half-height slots (see PIPE2_SLOTS), paired window and interleaved slots (pipe2_fill) ----
+    f2 *const P = pipe2_slots(smem, a.wrows, WP);
     if(tid < 2 * PIPE_SCAN_GROUP)
     {
       asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(cfg::SCAN_REGS));
@@ -1051,22 +1349,22 @@ __global__ void __launch_bounds__(pipe_cfg<CFG>::NT, 1) nlm_pipe_kernel(const __
         const bool live = t >= 1 && t < c.ncols;
         for(int q = group; q < npairs; q += 2)
         {
-          grp_colwalk_t<WP, R, NORM1> walk;
+          pipe2_colwalk_t<WP, NORM1> walk;
           if(live) walk.init(a, c, W, 2 * q, t);
 #pragma unroll
           for(int hh = 0; hh < 2; hh++)
           {
             const int w = 2 * q + hh, slot = w % PIPE2_SLOTS;
-            float *const Sa = S + slot * (2 * PIPE2_HSP) + t, *const Sb = Sa + PIPE2_HSP;
+            f2 *const Sp = P + slot * PIPE2_HSP + t;
             clk.mark(PIPE_ROLE_WORK);
             if(w >= PIPE2_SLOTS) named_sync(PIPE2_BAR_EMPTY + slot, PIPE2_A_T + PIPE2_ACC_HALF);
             clk.mark(PIPE_ROLE_EMPTY);
             if(live)
             {
               if(hh == 0)
-                walk.template half<0>(a, Sa, Sb);
+                walk.template half<0>(a, Sp);
               else
-                walk.template half<(PIPE2_HROWS % 3)>(a, Sa, Sb);
+                walk.template half<(PIPE2_HROWS % 3)>(a, Sp);
             }
             clk.mark(PIPE_ROLE_WORK);
             named_sync(PIPE2_BAR_HANDOVER + group, PIPE_SCAN_GROUP);
@@ -1084,7 +1382,7 @@ __global__ void __launch_bounds__(pipe_cfg<CFG>::NT, 1) nlm_pipe_kernel(const __
             clk.mark(PIPE_ROLE_WORK);
             named_sync(PIPE2_BAR_HANDOVER + group, PIPE_SCAN_GROUP);
             clk.mark(PIPE_ROLE_HANDOVER);
-            pipe2_b1<R>(a, c, S + slot * (2 * PIPE2_HSP), 2 * q, l);
+            pipe2_b1_rows<R>(c, P + slot * PIPE2_HSP, l);
             named_arrive(PIPE2_BAR_FULL + slot, 32 + PIPE2_ACC_HALF);
           }
       }
@@ -1096,17 +1394,16 @@ __global__ void __launch_bounds__(pipe_cfg<CFG>::NT, 1) nlm_pipe_kernel(const __
       asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(cfg::ACC_REGS));
       const int ta = tid - 2 * PIPE_SCAN_GROUP, hh = ta / PIPE2_ACC_HALF;
       grp_strip_t<cfg::KP, cfg::L, cfg::IL> st;
-      grp_own_init<WP>(a, c, W, st, ta);
-      st.sofs0 -= hh * PIPE2_HROWS * GRP_SP; // the planes of a slot start at the half's first row
+      pipe2_own_init<WP>(a, c, W, st, ta);
+      st.sofs0 -= hh * PIPE2_HROWS * GRP_SP; // the plane of a slot starts at the half's first row
       for(int q = 0; q < npairs; q++)
       {
         const int w = 2 * q + hh, slot = w % PIPE2_SLOTS;
-        const float *const Sa = S + slot * (2 * PIPE2_HSP);
         clk.mark(PIPE_ROLE_WORK);
         named_sync(PIPE2_BAR_FULL + slot, 32 + PIPE2_ACC_HALF);
         clk.mark(PIPE_ROLE_FULL);
-        grp_accumulate_pairs<WP, PROFILED, DIVC>(a, W + shifts[2 * q], Sa, st);
-        if(2 * q + 1 < a.n_patches) grp_accumulate_pairs<WP, PROFILED, DIVC>(a, W + shifts[2 * q + 1], Sa + PIPE2_HSP, st);
+        const bool both = 2 * q + 1 < a.n_patches;
+        pipe2_accumulate<WP, PROFILED, DIVC>(a, W, P + slot * PIPE2_HSP, shifts[2 * q], shifts[both ? 2 * q + 1 : 2 * q], both, st);
         if(w + PIPE2_SLOTS < 2 * npairs) named_arrive(PIPE2_BAR_EMPTY + slot, PIPE2_A_T + PIPE2_ACC_HALF);
       }
       clk.mark(PIPE_ROLE_WORK);
