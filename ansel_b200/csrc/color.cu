@@ -276,39 +276,6 @@ int color_process_dev(const b200_piece_t *piece, const b200_conversion_t *conv, 
     return passthrough(d_in, d_out, w * h * 4 * sizeof(float), (cudaStream_t)stream);
   return b200_apply_conversion_dev(conv, d_in, d_out, w, h, piece->mask_display & B200_DISPLAY_MASK, stream);
 }
-
-int color_process_host(const b200_piece_t *piece, const b200_conversion_t *conv, int type, const void *in, void *out)
-{
-  int rc = bind_device(piece->devid);
-  if(rc) return rc;
-  const size_t bytes = (size_t)piece->roi_out.width * piece->roi_out.height * 4 * sizeof(float);
-  void *d_in = nullptr, *d_out = nullptr;
-  cudaStream_t s;
-  if((rc = host_stream(&s))) return rc;
-  if((rc = scratch(SLOT_IN, bytes, &d_in))) return rc;
-  if((rc = scratch(SLOT_OUT, bytes, &d_out))) return rc;
-  if((rc = copy_h2d(d_in, in, bytes, s))) return rc;
-  if((rc = color_process_dev(piece, conv, type, d_in, d_out, (void *)s))) return rc;
-  if((rc = copy_d2h(out, d_out, bytes, s))) return rc;
-  B200_CUDA_TRY(cudaStreamSynchronize(s));
-  return B200_OK;
-}
-
-void default_tiling(const b200_piece_t *piece, b200_tiling_t *t)
-{
-  // default_tiling_callback(), develop/tiling.c:1423-1463, for modules placed after demosaic
-  if(!piece || !t) return;
-  const float ioratio = ((float)piece->roi_out.width * (float)piece->roi_out.height)
-                        / ((float)piece->roi_in.width * (float)piece->roi_in.height);
-  t->factor = 1.0f + ioratio;
-  t->factor_cl = t->factor;
-  t->maxbuf = 1.0f;
-  t->maxbuf_cl = 1.0f;
-  t->overhead = 0;
-  t->overlap = 0;
-  t->xalign = 1;
-  t->yalign = 1;
-}
 } // namespace
 
 #define COLOR_CHECK(op, T)                                                                         \
@@ -326,7 +293,8 @@ extern "C" int b200_colorin_process_host(const b200_piece_t *piece, const void *
 {
   COLOR_CHECK("colorin", b200_colorin_data_t)
   if(d->blue_mapping) return fail(B200_ERR_UNSUPPORTED, "colorin: the legacy blue-mapping hook (v1/v2 history) is not built");
-  return color_process_host(piece, d->conversion, d->type, in, out);
+  const size_t bytes = (size_t)piece->roi_out.width * piece->roi_out.height * 16;
+  return through_device(piece, in, bytes, out, bytes, false, b200_colorin_process_dev);
 }
 extern "C" int b200_colorout_process_dev(const b200_piece_t *piece, const void *in, void *out, void *stream)
 {
@@ -345,10 +313,12 @@ extern "C" int b200_colorout_process_scatter_dev(const b200_piece_t *piece, cons
 extern "C" int b200_colorout_process_host(const b200_piece_t *piece, const void *in, void *out)
 {
   COLOR_CHECK("colorout", b200_colorout_data_t)
-  return color_process_host(piece, d->conversion, d->type, in, out);
+  (void)d;
+  const size_t bytes = (size_t)piece->roi_out.width * piece->roi_out.height * 16;
+  return through_device(piece, in, bytes, out, bytes, false, b200_colorout_process_dev);
 }
-extern "C" void b200_colorin_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t); }
-extern "C" void b200_colorout_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t); }
+extern "C" void b200_colorin_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t, 0, false); }
+extern "C" void b200_colorout_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t, 0, false); }
 
 // dt_ioppr_init_unbounded_coeffs(), colorprofiles/iop_profile.c:303-329, with dt_iop_estimate_exp
 // (develop/imageop_math.h:135-165) and extrapolate_lut (iop_profile.h:536-545).  Host-side set-up

@@ -169,26 +169,14 @@ extern "C" int b200_demosaic_process_host(const b200_piece_t *piece, const void 
 {
   int rc = check_piece(piece, in, out);
   if(rc) return rc;
-  rc = bind_device(piece->devid);
-  if(rc) return rc;
-  const size_t npx_in = (size_t)piece->roi_in.width * piece->roi_in.height;
-  const size_t npx_out = (size_t)piece->roi_out.width * piece->roi_out.height;
-  void *d_in = nullptr, *d_out = nullptr;
-  cudaStream_t s;
-  if((rc = host_stream(&s))) return rc;
-  if((rc = scratch(SLOT_IN, npx_in * sizeof(float), &d_in))) return rc;
-  if((rc = scratch(SLOT_OUT, npx_out * 4 * sizeof(float), &d_out))) return rc;
-  if((rc = copy_h2d(d_in, in, npx_in * sizeof(float), s))) return rc;
   // The caller's cacheline may hold anything; the reference leaves the alpha of the outer 3 px
   // and (for frames under 16 px) the whole buffer as found.  Start from the caller's bytes only
   // in the too-small case and for PPG (which, like the reference, keeps the alpha of the outer three pixels);
   // otherwise every pixel is overwritten.
-  if(piece->roi_in.width < 16 || piece->roi_in.height < 16 || keeps_alpha(((const b200_demosaic_data_t *)piece->data)->demosaicing_method))
-    if((rc = copy_h2d(d_out, out, npx_out * 4 * sizeof(float), s))) return rc;
-  if((rc = b200_demosaic_process_dev(piece, d_in, d_out, (void *)s))) return rc;
-  if((rc = copy_d2h(out, d_out, npx_out * 4 * sizeof(float), s))) return rc;
-  B200_CUDA_TRY(cudaStreamSynchronize(s));
-  return B200_OK;
+  const bool carry_out = piece->roi_in.width < 16 || piece->roi_in.height < 16
+                         || keeps_alpha(((const b200_demosaic_data_t *)piece->data)->demosaicing_method);
+  return through_device(piece, in, (size_t)piece->roi_in.width * piece->roi_in.height * sizeof(float), out,
+                        (size_t)piece->roi_out.width * piece->roi_out.height * 4 * sizeof(float), carry_out, b200_demosaic_process_dev);
 }
 
 // tiling_callback(), iop/demosaic.c:1916-2013 (Bayer branches for the methods built here)

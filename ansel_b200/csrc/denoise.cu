@@ -709,18 +709,8 @@ extern "C" int b200_denoiseprofile_process_host(const b200_piece_t *piece, const
 {
   int rc = check_dn(piece, in, out);
   if(rc) return rc;
-  if((rc = bind_device(piece->devid))) return rc;
   const size_t bytes = (size_t)piece->roi_out.width * piece->roi_out.height * 16;
-  void *d_in = nullptr, *d_out = nullptr;
-  cudaStream_t s;
-  if((rc = host_stream(&s))) return rc;
-  if((rc = scratch(SLOT_IN, bytes, &d_in))) return rc;
-  if((rc = scratch(SLOT_OUT, bytes, &d_out))) return rc;
-  if((rc = copy_h2d(d_in, in, bytes, s))) return rc;
-  if((rc = b200_denoiseprofile_process_dev(piece, d_in, d_out, (void *)s))) return rc;
-  if((rc = copy_d2h(out, d_out, bytes, s))) return rc;
-  B200_CUDA_TRY(cudaStreamSynchronize(s));
-  return B200_OK;
+  return through_device(piece, in, bytes, out, bytes, false, b200_denoiseprofile_process_dev);
 }
 
 // tiling_callback(), denoiseprofile.c:796-849

@@ -344,31 +344,9 @@ extern "C" int b200_dither_process_host(const b200_piece_t *piece, const void *i
 {
   int rc = dither_check(piece, in, out);
   if(rc) return rc;
-  if((rc = bind_device(piece->devid))) return rc;
   const size_t bytes = (size_t)piece->roi_in.width * piece->roi_in.height * 16;
-  void *d_in = nullptr, *d_out = nullptr;
-  cudaStream_t s;
-  if((rc = host_stream(&s))) return rc;
-  if((rc = scratch(SLOT_IN, bytes, &d_in))) return rc;
-  if((rc = scratch(SLOT_OUT, bytes, &d_out))) return rc;
-  if((rc = copy_h2d(d_in, in, bytes, s))) return rc;
-  if((rc = b200_dither_process_dev(piece, d_in, d_out, (void *)s))) return rc;
-  if((rc = copy_d2h(out, d_out, bytes, s))) return rc;
-  B200_CUDA_TRY(cudaStreamSynchronize(s));
-  return B200_OK;
+  return through_device(piece, in, bytes, out, bytes, false, b200_dither_process_dev);
 }
 
-extern "C" void b200_dither_tiling(const b200_piece_t *piece, b200_tiling_t *t)
-{ // no tiling_callback of its own: default_tiling_callback, develop/tiling.c:1423-1463
-  if(!piece || !t) return;
-  const float ioratio = ((float)piece->roi_out.width * (float)piece->roi_out.height) / ((float)piece->roi_in.width * (float)piece->roi_in.height);
-  t->factor = 1.0f + ioratio;
-  t->factor_cl = t->factor;
-  t->maxbuf = 1.0f;
-  t->maxbuf_cl = 1.0f;
-  t->overhead = 0;
-  t->overlap = 0;
-  t->xalign = 1;
-  t->yalign = 1;
-}
+extern "C" void b200_dither_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t, 0, false); } // the module declares no tiling callback
 #endif

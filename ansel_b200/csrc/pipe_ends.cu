@@ -826,42 +826,6 @@ int launch_front(const void *d_in, void *d_out, int width, int height, const pre
   B200_CUDA_TRY(cudaGetLastError());
   return B200_OK;
 }
-
-// host-pointer wrapper shared by every module of this file
-typedef int (*dev_fn)(const b200_piece_t *, const void *, void *, void *);
-int through_device(const b200_piece_t *piece, const void *in, void *out, size_t in_bytes, size_t out_bytes, dev_fn fn, bool out_is_read)
-{
-  int rc = bind_device(piece->devid);
-  if(rc) return rc;
-  void *d_in = nullptr, *d_out = nullptr;
-  cudaStream_t s;
-  if((rc = host_stream(&s))) return rc;
-  if((rc = scratch(SLOT_IN, in_bytes, &d_in))) return rc;
-  if((rc = scratch(SLOT_OUT, out_bytes, &d_out))) return rc;
-  if((rc = copy_h2d(d_in, in, in_bytes, s))) return rc;
-  if(out_is_read && (rc = copy_h2d(d_out, out, out_bytes, s))) return rc;
-  if((rc = fn(piece, d_in, d_out, (void *)s))) return rc;
-  if((rc = copy_d2h(out, d_out, out_bytes, s))) return rc;
-  B200_CUDA_TRY(cudaStreamSynchronize(s));
-  return B200_OK;
-}
-
-// default_tiling_callback(), develop/tiling.c:1423-1463; full_roi: IOP_FLAGS_TILING_FULL_ROI; raw: placed before demosaic
-void default_tiling(const b200_piece_t *piece, b200_tiling_t *t, bool full_roi, bool raw)
-{
-  if(!piece || !t) return;
-  const float ioratio = ((float)piece->roi_out.width * (float)piece->roi_out.height) / ((float)piece->roi_in.width * (float)piece->roi_in.height);
-  t->factor = 1.0f + ioratio;
-  t->factor_cl = t->factor;
-  t->maxbuf = 1.0f;
-  t->maxbuf_cl = 1.0f;
-  t->overhead = 0;
-  t->overlap = full_roi ? 4 : 0;
-  t->xalign = 1;
-  t->yalign = 1;
-  if(!raw || !piece->filters) return;
-  t->xalign = t->yalign = (piece->filters == 9u) ? 3 : 2;
-}
 } // namespace
 
 // ---- rawprepare ------------------------------------------------------------------------------------------------------------
@@ -895,10 +859,10 @@ extern "C" int b200_rawprepare_process_host(const b200_piece_t *piece, const voi
 {
   int rc = check_piece("rawprepare", piece, in, out, sizeof(b200_rawprepare_data_t));
   if(rc) return rc;
-  return through_device(piece, in, out, rawprepare_in_bytes(piece), (size_t)piece->roi_out.width * piece->roi_out.height * 4 * piece->channels,
-                        b200_rawprepare_process_dev, false);
+  return through_device(piece, in, rawprepare_in_bytes(piece), out, (size_t)piece->roi_out.width * piece->roi_out.height * 4 * piece->channels, false,
+                        b200_rawprepare_process_dev);
 }
-extern "C" void b200_rawprepare_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t, true, true); }
+extern "C" void b200_rawprepare_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t, 4, true); }
 
 // ---- temperature -------------------------------------------------------------------------------------------------------------
 extern "C" int b200_temperature_process_dev(const b200_piece_t *piece, const void *d_in, void *d_out, void *stream)
@@ -949,9 +913,9 @@ extern "C" int b200_temperature_process_host(const b200_piece_t *piece, const vo
   if(rc) return rc;
   const size_t bytes = (size_t)piece->roi_out.width * piece->roi_out.height * 4 * (piece->filters ? 1 : piece->channels);
   // channel counts other than 4 leave part of every output pixel unwritten: carry what the caller's buffer holds
-  return through_device(piece, in, out, bytes, bytes, b200_temperature_process_dev, !piece->filters && piece->channels != 4);
+  return through_device(piece, in, bytes, out, bytes, !piece->filters && piece->channels != 4, b200_temperature_process_dev);
 }
-extern "C" void b200_temperature_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t, false, true); }
+extern "C" void b200_temperature_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t, 0, true); }
 
 // ---- highlights --------------------------------------------------------------------------------------------------------------
 // colour inpainting, both mosaics: the mosaic transposed, the two row directions on the copy and the two column directions on the frame, the row
@@ -1100,7 +1064,7 @@ extern "C" int b200_highlights_process_host(const b200_piece_t *piece, const voi
   int rc = check_piece("highlights", piece, in, out, sizeof(b200_highlights_data_t));
   if(rc) return rc;
   const size_t bytes = (size_t)piece->roi_out.width * piece->roi_out.height * 4 * (piece->filters ? 1 : piece->channels);
-  return through_device(piece, in, out, bytes, bytes, b200_highlights_process_dev, false);
+  return through_device(piece, in, bytes, out, bytes, false, b200_highlights_process_dev);
 }
 extern "C" void b200_highlights_tiling(const b200_piece_t *piece, b200_tiling_t *t)
 { // highlights.c:575-644
@@ -1215,9 +1179,9 @@ extern "C" int b200_exposure_process_host(const b200_piece_t *piece, const void 
   int rc = check_piece("exposure", piece, in, out, sizeof(b200_exposure_data_t));
   if(rc) return rc;
   const size_t bytes = (size_t)piece->roi_out.width * piece->roi_out.height * 4 * piece->channels;
-  return through_device(piece, in, out, bytes, bytes, b200_exposure_process_dev, false);
+  return through_device(piece, in, bytes, out, bytes, false, b200_exposure_process_dev);
 }
-extern "C" void b200_exposure_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t, false, false); }
+extern "C" void b200_exposure_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t, 0, false); }
 
 // ---- gamma and the export conversions -------------------------------------------------------------------------------------------
 extern "C" int b200_gamma_process_dev(const b200_piece_t *piece, const void *d_in, void *d_out, void *stream)
@@ -1236,9 +1200,9 @@ extern "C" int b200_gamma_process_host(const b200_piece_t *piece, const void *in
   int rc = check_piece("gamma", piece, in, out, 0);
   if(rc) return rc;
   const size_t npx = (size_t)piece->roi_out.width * piece->roi_out.height;
-  return through_device(piece, in, out, npx * 16, npx * 4, b200_gamma_process_dev, true); // the fourth byte of every pixel is the caller's
+  return through_device(piece, in, npx * 16, out, npx * 4, true, b200_gamma_process_dev); // the fourth byte of every pixel is the caller's
 }
-extern "C" void b200_gamma_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t, false, false); }
+extern "C" void b200_gamma_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t, 0, false); }
 
 extern "C" int b200_export_convert_dev(const void *d_in, void *d_out, size_t width, size_t height, int format, void *stream)
 {
@@ -1260,18 +1224,8 @@ extern "C" int b200_export_convert_host(const void *in, void *out, size_t width,
 {
   if(!in || !out || !width || !height) return fail(B200_ERR_ARG, "export_convert: NULL or empty argument");
   if(format < B200_EXPORT_UINT8 || format > B200_EXPORT_UINT16) return fail(B200_ERR_ARG, "export_convert: format %d", format);
-  int rc = bind_device(-1);
-  if(rc) return rc;
-  const size_t npx = width * height, out_bytes = npx * (format == B200_EXPORT_UINT16 ? 8 : 4);
-  void *d_in = nullptr, *d_out = nullptr;
-  cudaStream_t s;
-  if((rc = host_stream(&s))) return rc;
-  if((rc = scratch(SLOT_IN, npx * 16, &d_in))) return rc;
-  if((rc = scratch(SLOT_OUT, out_bytes, &d_out))) return rc;
-  if((rc = copy_h2d(d_in, in, npx * 16, s))) return rc;
-  if((rc = b200_export_convert_dev(d_in, d_out, width, height, format, (void *)s))) return rc;
-  if((rc = copy_d2h(out, d_out, out_bytes, s))) return rc;
-  B200_CUDA_TRY(cudaStreamSynchronize(s));
-  return B200_OK;
+  const size_t npx = width * height;
+  return through_device(-1, in, npx * 16, out, npx * (format == B200_EXPORT_UINT16 ? 8 : 4), false,
+                        [=](const void *d_in, void *d_out, void *stream) { return b200_export_convert_dev(d_in, d_out, width, height, format, stream); });
 }
 #endif // B200_KERNELS_ON_CPU

@@ -277,46 +277,34 @@ static int clip_and_zoom_dev(const b200_piece_t *piece, const void *d_in, void *
   return B200_OK;
 }
 
-static int clip_and_zoom_host(const b200_piece_t *piece, const void *in, void *out, bool keep_origins);
-extern "C" int b200_finalscale_process_host(const b200_piece_t *piece, const void *in, void *out) { return clip_and_zoom_host(piece, in, out, false); }
-extern "C" int b200_initialscale_process_host(const b200_piece_t *piece, const void *in, void *out) { return clip_and_zoom_host(piece, in, out, true); }
-static int clip_and_zoom_host(const b200_piece_t *piece, const void *in, void *out, bool keep_origins)
+static int check_zoom(const b200_piece_t *piece, const void *in, const void *out)
 {
   if(!piece || !in || !out) return fail(B200_ERR_ARG, "finalscale: NULL argument");
   if(piece->roi_in.width < 1 || piece->roi_in.height < 1 || piece->roi_out.width < 1 || piece->roi_out.height < 1)
     return fail(B200_ERR_ARG, "finalscale: empty ROI");
-  int rc = bind_device(piece->devid);
-  if(rc) return rc;
-  const size_t in_bytes = (size_t)piece->roi_in.width * piece->roi_in.height * 16, out_bytes = (size_t)piece->roi_out.width * piece->roi_out.height * 16;
-  void *d_in = nullptr, *d_out = nullptr;
-  cudaStream_t s;
-  if((rc = host_stream(&s))) return rc;
-  if((rc = scratch(SLOT_IN, in_bytes, &d_in))) return rc;
-  if((rc = scratch(SLOT_OUT, out_bytes, &d_out))) return rc;
-  if((rc = copy_h2d(d_in, in, in_bytes, s))) return rc;
-  if((rc = clip_and_zoom_dev(piece, d_in, d_out, (void *)s, keep_origins))) return rc;
-  if((rc = copy_d2h(out, d_out, out_bytes, s))) return rc;
-  B200_CUDA_TRY(cudaStreamSynchronize(s));
   return B200_OK;
 }
-
-extern "C" void b200_finalscale_tiling(const b200_piece_t *piece, b200_tiling_t *t)
-{ // no tiling_callback of its own: default_tiling_callback (develop/tiling.c:1423-1463) with IOP_FLAGS_TILING_FULL_ROI
-  if(!piece || !t) return;
-  const float ioratio = ((float)piece->roi_out.width * (float)piece->roi_out.height) / ((float)piece->roi_in.width * (float)piece->roi_in.height);
-  t->factor = 1.0f + ioratio;
-  t->factor_cl = t->factor;
-  t->maxbuf = 1.0f;
-  t->maxbuf_cl = 1.0f;
-  t->overhead = 0;
-  t->overlap = 4;
-  t->xalign = 1;
-  t->yalign = 1;
+extern "C" int b200_finalscale_process_host(const b200_piece_t *piece, const void *in, void *out)
+{
+  int rc = check_zoom(piece, in, out);
+  if(rc) return rc;
+  const size_t in_bytes = (size_t)piece->roi_in.width * piece->roi_in.height * 16, out_bytes = (size_t)piece->roi_out.width * piece->roi_out.height * 16;
+  return through_device(piece, in, in_bytes, out, out_bytes, false, b200_finalscale_process_dev);
 }
+extern "C" int b200_initialscale_process_host(const b200_piece_t *piece, const void *in, void *out)
+{
+  int rc = check_zoom(piece, in, out);
+  if(rc) return rc;
+  const size_t in_bytes = (size_t)piece->roi_in.width * piece->roi_in.height * 16, out_bytes = (size_t)piece->roi_out.width * piece->roi_out.height * 16;
+  return through_device(piece, in, in_bytes, out, out_bytes, false, b200_initialscale_process_dev);
+}
+
+// neither module declares a tiling callback; both have IOP_FLAGS_TILING_FULL_ROI
+extern "C" void b200_finalscale_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t, 4, false); }
 #endif // B200_KERNELS_ON_CPU
 
 #ifndef B200_KERNELS_ON_CPU
-extern "C" void b200_initialscale_tiling(const b200_piece_t *piece, b200_tiling_t *t) { b200_finalscale_tiling(piece, t); } // same flags, no callback of its own
+extern "C" void b200_initialscale_tiling(const b200_piece_t *piece, b200_tiling_t *t) { default_tiling(piece, t, 4, false); }
 
 // ---- flip -------------------------------------------------------------------------------------------------------------------------
 extern "C" int b200_flip_process_dev(const b200_piece_t *piece, const void *d_in, void *d_out, void *stream)
@@ -338,19 +326,8 @@ extern "C" int b200_flip_process_host(const b200_piece_t *piece, const void *in,
 {
   if(!piece || !in || !out) return fail(B200_ERR_ARG, "flip: NULL argument");
   if(piece->roi_in.width < 1 || piece->roi_in.height < 1 || piece->channels < 1) return fail(B200_ERR_ARG, "flip: empty ROI");
-  int rc = bind_device(piece->devid);
-  if(rc) return rc;
   const size_t bytes = (size_t)piece->roi_in.width * piece->roi_in.height * piece->channels * sizeof(float);
-  void *d_in = nullptr, *d_out = nullptr;
-  cudaStream_t s;
-  if((rc = host_stream(&s))) return rc;
-  if((rc = scratch(SLOT_IN, bytes, &d_in))) return rc;
-  if((rc = scratch(SLOT_OUT, bytes, &d_out))) return rc;
-  if((rc = copy_h2d(d_in, in, bytes, s))) return rc;
-  if((rc = b200_flip_process_dev(piece, d_in, d_out, (void *)s))) return rc;
-  if((rc = copy_d2h(out, d_out, bytes, s))) return rc;
-  B200_CUDA_TRY(cudaStreamSynchronize(s));
-  return B200_OK;
+  return through_device(piece, in, bytes, out, bytes, false, b200_flip_process_dev);
 }
 extern "C" void b200_flip_tiling(const b200_piece_t *piece, b200_tiling_t *t)
 { // flip.c tiling_callback: in + out, no overlap; the module does not define alignment

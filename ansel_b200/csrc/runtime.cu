@@ -1,4 +1,5 @@
-// libb200iop.so runtime: errors, device binding, per-thread scratch, host<->device staging.
+// libb200iop.so runtime: errors, device binding, per-thread scratch, host<->device staging, the host entries' round trip, the
+// default tiling callback.
 // Counterpart of the reference's OpenCL runtime (src/common/opencl.c) for CUDA on H100.
 #include "runtime.h"
 #include <vector>
@@ -241,6 +242,46 @@ int copy_d2h(void *dst, const void *src, size_t bytes, cudaStream_t stream)
   }
   (void)done;
   return B200_OK;
+}
+
+int through_device(int devid, const void *in, size_t in_bytes, void *out, size_t out_bytes, bool carry_out,
+                   const std::function<int(const void *d_in, void *d_out, void *stream)> &run)
+{
+  int rc = bind_device(devid);
+  if(rc) return rc;
+  void *d_in = nullptr, *d_out = nullptr;
+  cudaStream_t s;
+  if((rc = host_stream(&s))) return rc;
+  if((rc = scratch(SLOT_IN, in_bytes, &d_in))) return rc;
+  if((rc = scratch(SLOT_OUT, out_bytes, &d_out))) return rc;
+  if((rc = copy_h2d(d_in, in, in_bytes, s))) return rc;
+  if(carry_out && (rc = copy_h2d(d_out, out, out_bytes, s))) return rc;
+  if((rc = run(d_in, d_out, (void *)s))) return rc;
+  if((rc = copy_d2h(out, d_out, out_bytes, s))) return rc;
+  B200_CUDA_TRY(cudaStreamSynchronize(s));
+  return B200_OK;
+}
+
+int through_device(const b200_piece_t *piece, const void *in, size_t in_bytes, void *out, size_t out_bytes, bool carry_out, dev_fn fn)
+{
+  return through_device(piece->devid, in, in_bytes, out, out_bytes, carry_out,
+                        [=](const void *d_in, void *d_out, void *stream) { return fn(piece, d_in, d_out, stream); });
+}
+
+void default_tiling(const b200_piece_t *piece, b200_tiling_t *t, unsigned overlap, bool raw)
+{
+  if(!piece || !t) return;
+  const float ioratio = ((float)piece->roi_out.width * (float)piece->roi_out.height) / ((float)piece->roi_in.width * (float)piece->roi_in.height);
+  t->factor = 1.0f + ioratio;
+  t->factor_cl = t->factor;
+  t->maxbuf = 1.0f;
+  t->maxbuf_cl = 1.0f;
+  t->overhead = 0;
+  t->overlap = overlap;
+  t->xalign = 1;
+  t->yalign = 1;
+  if(!raw || !piece->filters) return;
+  t->xalign = t->yalign = (piece->filters == 9u) ? 3 : 2;
 }
 // ---- launch timing of the headline kernels ----------------------------------------------------------------
 namespace

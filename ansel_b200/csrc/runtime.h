@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
+#include <functional>
 #include "../../include/b200iop.h"
 
 namespace b200
@@ -51,6 +52,21 @@ int copy_d2h(void *dst, const void *src, size_t bytes, cudaStream_t stream);
 
 // per-thread non-blocking stream used by the *_process_host entry points
 int host_stream(cudaStream_t *s);
+
+// The body of every b200_<op>_process_host(), run after the module has checked its arguments: bind the device, upload
+// `in_bytes` of `in` (and, with carry_out, the caller's `out` too, for modules that leave part of their output as they find
+// it), run the module's _dev entry on the thread's host stream, download `out_bytes` into `out` and synchronise.  `out` is
+// not written unless the _dev entry succeeded.
+typedef int (*dev_fn)(const b200_piece_t *piece, const void *d_in, void *d_out, void *stream);
+int through_device(const b200_piece_t *piece, const void *in, size_t in_bytes, void *out, size_t out_bytes, bool carry_out, dev_fn fn);
+// the same for an entry point without a piece: `run` gets the device buffers and the stream
+int through_device(int devid, const void *in, size_t in_bytes, void *out, size_t out_bytes, bool carry_out,
+                   const std::function<int(const void *d_in, void *d_out, void *stream)> &run);
+
+// default_tiling_callback(), develop/tiling.c:1423-1463, for the modules that declare no tiling callback: factor 1 + the
+// roi_out / roi_in area ratio, no overhead; `overlap` 4 for IOP_FLAGS_TILING_FULL_ROI, else 0; `raw` (placed before
+// demosaic) aligns tiles on the mosaic's pattern, 2 px on Bayer sensors and 3 on X-Trans.
+void default_tiling(const b200_piece_t *piece, b200_tiling_t *t, unsigned overlap, bool raw);
 
 // Launch timing of the headline kernels (b200_kernel_timing, b200_kernel_timing_read): when enabled, a pair of CUDA
 // events brackets the launch on the stream it goes to.  One `if` per launch when disabled.

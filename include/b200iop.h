@@ -2,7 +2,7 @@
  *
  * Drop-in boundary (SURVEY.md section 8b).  A reference module keeps its dt_iop_module_t
  * surface (src/iop/iop_api.h:80-351) in plain C and forwards the body of
- *     process()            iop_api.h:265-266   -> b200_<op>_process_host()   host pointers, H2D + kernels + D2H
+ *     process()            iop_api.h:265-266   -> b200_<op>_process_host()   host pointers: upload, _dev, download
  *     process_cl()         iop_api.h:292-293   -> b200_<op>_process_dev()    device pointers + stream, no copies
  *     tiling_callback()    iop_api.h:121-122   -> b200_<op>_tiling()
  * to this library.  ansel_b200/iop/ holds those C adapters; INTEGRATION.md shows where they slot
@@ -243,7 +243,9 @@ int b200_colorin_process_host(const b200_piece_t *piece, const void *in, void *o
 int b200_colorin_process_dev(const b200_piece_t *piece, const void *d_in, void *d_out, void *stream);
 int b200_colorout_process_host(const b200_piece_t *piece, const void *in, void *out);
 int b200_colorout_process_dev(const b200_piece_t *piece, const void *d_in, void *d_out, void *stream);
-/* default_tiling_callback(), develop/tiling.c:1423-1463: factor 2, no overlap */
+/* default_tiling_callback(), develop/tiling.c:1423-1463, as every module without a tiling callback of its own answers here:
+ * factor 1 + roi_out area / roi_in area, maxbuf 1, no overhead, overlap 4 with IOP_FLAGS_TILING_FULL_ROI (else 0), tiles
+ * aligned on the mosaic's pattern (2 px Bayer, 3 px X-Trans) for the modules before demosaic (else 1) */
 void b200_colorin_tiling(const b200_piece_t *piece, b200_tiling_t *tiling);
 void b200_colorout_tiling(const b200_piece_t *piece, b200_tiling_t *tiling);
 /* dt_colorspaces_apply_conversion(), colorprofiles/conversion.c:762-766, on device buffers */
