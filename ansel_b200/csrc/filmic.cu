@@ -16,6 +16,26 @@
 // Roofline: 32 B/px of HBM traffic against ~3 log2f + up to 9 powf (each a double-precision
 // polynomial) + 5 sqrtf + ~30 IEEE divisions per pixel: FP64/XU-issue bound by an order of magnitude,
 // not HBM bound (SURVEY.md 8d); reported as such.
+//
+// Code shape of filmic_agx_kernel.  Every helper was already inlined; what cost time was the size of the code and two arrays in
+// local memory.  Steps, each on top of the previous one, timed by tools/time_filmic.py (the bench frame, v8 defaults with the export
+// profile, median of 3 alternating rounds of 15 calls, outputs byte-identical) on an H100 80GB HBM3 at 700 W, 1980 MHz; SASS of the
+// export instance (sm_90a, CUDA 12.9):
+//
+//   step                                                       instr  stack  LDL/STL  CALL  BSSY  regs   time
+//   parent                                                      6512   32 B   41/20    158   272    38   4.37 ms
+//   A  powf_special() returns by value; the tone loop rotates   6376    0      0/0     158   270    52   4.54 ms
+//      its three channels through registers
+//   B  + use_output_profile a template parameter                4288    0      0/0      96   173    46   4.45 ms
+//   C  + one rolled copy of the three clip_white / clip_black,  2520    0      0/0      40    90    45   3.22 ms
+//      one clip_white_raw per clip_white
+//   D  + __launch_bounds__(128, 12): 40 registers, 48 warps     2520    0      0/0      40    90    38   3.14 ms
+//
+// A and B alone were slower: they raised the register count (36 resident warps per SM instead of 48) and saved little issue.  C
+// paid: the three clip rows had been six inlined clip_white_raw and three clip_black, 41 % of B's code, and the kernel's code
+// fell from 104 KB (parent) to 40 KB.  D gave back the occupancy.  All four are kept: D needs A's registers freed
+// and C's smaller body.  What remains is divergence across the spline segments and the clip branches, which a pointwise kernel
+// has no other pixel map to avoid, and the issue of the divisions and the FP64 libm cores.
 #include "runtime.h"
 #include <stddef.h>
 #include "flt32_math.cuh"
@@ -353,11 +373,10 @@ __device__ __forceinline__ float clip_white(const float co[4], float tw, float Y
   const float eps = 1e-3f;
   const float max_Y = Y31_TO_Y06(tw);
   const float delta_Y = MAXF(max_Y - Y, 0.f);
-  float mc;
-  if(delta_Y < eps)
-    mc = delta_Y / (eps * max_Y) * clip_white_raw(co, tw, (1.f - eps) * max_Y, ch, sh);
-  else
-    mc = clip_white_raw(co, tw, Y, ch, sh);
+  // both branches of the reference evaluate clip_white_raw(), at different Y: one inlined copy serves them
+  const bool near_white = delta_Y < eps;
+  const float raw = clip_white_raw(co, tw, near_white ? (1.f - eps) * max_Y : Y, ch, sh);
+  const float mc = near_white ? delta_Y / (eps * max_Y) * raw : raw;
   return mc >= 0.f ? mc : FLT_MAX;
 }
 __device__ __forceinline__ float clip_black(const float co[4], float ch, float sh)
@@ -371,8 +390,15 @@ __device__ __forceinline__ float clip_black(const float co[4], float ch, float s
 }
 __device__ __forceinline__ float clip_chroma(const float (*out_m)[4], float tw, float Y, float ch, float sh, float chroma)
 {
-  const float w = MINF(MINF(clip_white(out_m[0], tw, Y, ch, sh), clip_white(out_m[1], tw, Y, ch, sh)), clip_white(out_m[2], tw, Y, ch, sh));
-  const float b = MINF(MINF(clip_black(out_m[0], ch, sh), clip_black(out_m[1], ch, sh)), clip_black(out_m[2], ch, sh));
+  // one rolled copy of the clips serves the three rows of out_m; the folds keep the reference's order, MINF(MINF(r0, r1), r2)
+  float w = 0.f, b = 0.f;
+#pragma unroll 1
+  for(int i = 0; i < 3; i++)
+  {
+    const float wi = clip_white(out_m[i], tw, Y, ch, sh), bi = clip_black(out_m[i], ch, sh);
+    w = i == 0 ? wi : MINF(w, wi);
+    b = i == 0 ? bi : MINF(b, bi);
+  }
   return MINF(MINF(chroma, b), w);
 }
 __device__ void gamut_check_rgb(const float (*m_out)[4], const float (*m_in)[4], float black, float white, const float Ych[4], float out[4])
@@ -394,8 +420,11 @@ __device__ void gamut_check_rgb(const float (*m_out)[4], const float (*m_in)[4],
   for(int c = 0; c < 4; c++) out[c] = CLAMPG(out[c], 0.f, white);
 }
 
-// gamut_mapping_simd(), :1986-2030 (filmic_desaturate_v4 :1779-1816, gamut_check_Yrg_filmic_simd :1928-1946)
-__device__ void gamut_map(const filmic_args_t &a, float Yf[4], const float Yr[4], float saturation, float res[4])
+// gamut_mapping_simd(), :1986-2030 (filmic_desaturate_v4 :1779-1816, gamut_check_Yrg_filmic_simd :1928-1946).
+// EXPORT = a.use_output_profile, the same for every pixel of a launch: each kernel instance compiles one of the two
+// gamut checks.
+template <bool EXPORT>
+__device__ __forceinline__ void gamut_map(const filmic_args_t &a, float Yf[4], const float Yr[4], float saturation, float res[4])
 {
   Yf[2] = Yr[2];
   Yf[3] = Yr[3];
@@ -417,7 +446,7 @@ __device__ void gamut_map(const filmic_args_t &a, float Yf[4], const float Yr[4]
     if(y1 + y2 > 1.f) max_c = fminf((1.f - 0.21902143f - 0.54371398f) / (Yf[2] + Yf[3]), max_c);
     Yf[1] = max_c;
   }
-  if(!a.use_output_profile)
+  if(!EXPORT)
     gamut_check_rgb(a.output, a.input, a.black, a.white, Yf, res);
   else
   {
@@ -428,7 +457,9 @@ __device__ void gamut_map(const filmic_args_t &a, float Yf[4], const float Yr[4]
   }
 }
 
-__global__ void __launch_bounds__(128) filmic_agx_kernel(const float4 *__restrict__ in, float4 *__restrict__ out, size_t npx,
+// 12 blocks per SM hold the kernel at 40 registers and 48 resident warps; left free, ptxas takes 45 and 36 warps fit (step D above)
+template <bool EXPORT>
+__global__ void __launch_bounds__(128, 12) filmic_agx_kernel(const float4 *__restrict__ in, float4 *__restrict__ out, size_t npx,
                                                          const __grid_constant__ filmic_args_t a)
 {
   __shared__ double tabs[f32m::SMEM_DOUBLES];
@@ -475,13 +506,16 @@ __global__ void __launch_bounds__(128) filmic_agx_kernel(const float4 *__restric
   rgb_to_ych(cmp, a.input, Yo);
   float ren[4];
   mat4(a.inset, cmp, ren);
-  // RGB_tone_mapping_v4_simd(), :2133-2149
+  // RGB_tone_mapping_v4_simd(), :2133-2149.  One rolled copy of the curve serves the three channels; they rotate
+  // through ren[0..2] so that no array is indexed at run time (that would place it in local memory).
 #pragma unroll 1
   for(int c = 0; c < 3; c++)
   {
-    const float lg = fminf(fmaxf((f32m::log2f_(tb, ren[c] / a.grey_source) - a.black_source) / a.dynamic_range, 0.0f), 1.0f);
+    const float lg = fminf(fmaxf((f32m::log2f_(tb, ren[0] / a.grey_source) - a.black_source) / a.dynamic_range, 0.0f), 1.0f);
     const float sp = spline_eval(tb, lg, a.spline);
-    ren[c] = f32m::powf_(tb, CLAMPF(sp, 0.f, a.spline.y[4]), a.output_power);
+    ren[0] = ren[1];
+    ren[1] = ren[2];
+    ren[2] = f32m::powf_(tb, CLAMPF(sp, 0.f, a.spline.y[4]), a.output_power);
   }
   float po[4];
   mat4(a.outset, ren, po);
@@ -496,7 +530,7 @@ __global__ void __launch_bounds__(128) filmic_agx_kernel(const float4 *__restric
   Yf[1] = chroma_final;
 
   float res[4];
-  gamut_map(a, Yf, Yr, 0.f, res);
+  gamut_map<EXPORT>(a, Yf, Yr, 0.f, res);
   if(a.copy_alpha) res[3] = p.w; // dt_iop_alpha_copy when the pipe displays a mask (:2893-2894)
   __stcs(out + k, make_float4(res[0], res[1], res[2], res[3]));
 }
@@ -605,7 +639,10 @@ __global__ void __launch_bounds__(128) filmic_legacy_kernel(const float4 *__rest
     rgb_to_ych(pix, a.input, Yo);
     rgb_to_ych(po, a.input, Yf);
     if(clamp_chroma) Yf[1] = fminf(Yo[1], Yf[1]);
-    gamut_map(a, Yf, Yo, saturation, res);
+    if(a.use_output_profile)
+      gamut_map<true>(a, Yf, Yo, saturation, res);
+    else
+      gamut_map<false>(a, Yf, Yo, saturation, res);
   }
   else if(a.preserve_color == 0)
   { // filmic_split_v1 :1534-1571, filmic_split_v2_v3 :1575-1612; lane 3 is not written by the reference: the input's is kept
@@ -737,7 +774,8 @@ extern "C" int b200_filmicrgb_process_dev(const b200_piece_t *piece, const void 
   a.norm_max = d->grey_source * exp2f(d->dynamic_range * 1.f + d->black_source);
   for(int c = 0; c < 3; c++) a.work_lum[c] = fp->work_profile.matrix_in[1][c];
   if(d->version >= 5)
-    filmic_agx_kernel<<<(unsigned)((npx + 127) / 128), 128, 0, (cudaStream_t)stream>>>((const float4 *)d_in, (float4 *)d_out, npx, a);
+    (a.use_output_profile ? filmic_agx_kernel<true> : filmic_agx_kernel<false>)<<<(unsigned)((npx + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+      (const float4 *)d_in, (float4 *)d_out, npx, a);
   else
     filmic_legacy_kernel<<<(unsigned)((npx + 127) / 128), 128, 0, (cudaStream_t)stream>>>((const float4 *)d_in, (float4 *)d_out, npx, a);
   B200_CUDA_TRY(cudaGetLastError());

@@ -228,18 +228,27 @@ __device__ __forceinline__ int checkint(uint32_t iy)
 }
 __device__ __forceinline__ bool zeroinfnan(uint32_t ix) { return 2 * ix - 1 >= 2u * 0x7f800000u - 1; }
 
-// the rare inputs of powf: x < 0x1p-126, x inf/nan, y zero/inf/nan.  Returns true when `out` is
-// final; otherwise ix / sign_bias are prepared for the main path.
-static __device__ __noinline__ bool powf_special(float x, float y, uint32_t &ix, uint32_t iy, uint32_t &sign_bias, float &out)
+// the rare inputs of powf: x < 0x1p-126, x inf/nan, y zero/inf/nan.  `done` says `out` is final;
+// otherwise ix / sign_bias are prepared for the main path.  Everything travels by value: the call
+// is out of line, and an argument passed by reference would put ix and sign_bias on the stack, with
+// a store and three loads of local memory on every powf_ call, special or not.
+struct powf_pre_t
 {
+  float out;
+  uint32_t ix, sign_bias;
+  bool done;
+};
+static __device__ __noinline__ powf_pre_t powf_special(float x, float y, uint32_t ix, uint32_t iy)
+{
+  powf_pre_t r = { 0.0f, ix, 0u, true };
   if(zeroinfnan(iy))
   {
-    if(2 * iy == 0 || ix == 0x3f800000u) out = 1.0f;
-    else if(2 * ix > 2u * 0x7f800000u || 2 * iy > 2u * 0x7f800000u) out = x + y;
-    else if(2 * ix == 2 * 0x3f800000u) out = 1.0f;
-    else if((2 * ix < 2 * 0x3f800000u) == !(iy & 0x80000000u)) out = 0.0f;
-    else out = y * y;
-    return true;
+    if(2 * iy == 0 || ix == 0x3f800000u) r.out = 1.0f;
+    else if(2 * ix > 2u * 0x7f800000u || 2 * iy > 2u * 0x7f800000u) r.out = x + y;
+    else if(2 * ix == 2 * 0x3f800000u) r.out = 1.0f;
+    else if((2 * ix < 2 * 0x3f800000u) == !(iy & 0x80000000u)) r.out = 0.0f;
+    else r.out = y * y;
+    return r;
   }
   if(zeroinfnan(ix))
   {
@@ -250,28 +259,29 @@ static __device__ __noinline__ bool powf_special(float x, float y, uint32_t &ix,
       x2 = -x2;
       neg = true;
     }
-    if(2 * ix == 0 && (iy & 0x80000000u)) out = neg ? -CUDART_INF_F : CUDART_INF_F;
-    else out = (iy & 0x80000000u) ? 1.0f / x2 : x2;
-    return true;
+    if(2 * ix == 0 && (iy & 0x80000000u)) r.out = neg ? -CUDART_INF_F : CUDART_INF_F;
+    else r.out = (iy & 0x80000000u) ? 1.0f / x2 : x2;
+    return r;
   }
   if(ix & 0x80000000u)
   {
     const int yint = checkint(iy);
     if(yint == 0)
     {
-      out = CUDART_NAN_F;
-      return true;
+      r.out = CUDART_NAN_F;
+      return r;
     }
-    if(yint == 1) sign_bias = 1u << (5 + 11);
-    ix &= 0x7fffffffu;
+    if(yint == 1) r.sign_bias = 1u << (5 + 11);
+    r.ix &= 0x7fffffffu;
   }
-  if(ix < 0x00800000u)
+  if(r.ix < 0x00800000u)
   {
-    ix = __float_as_uint(x * 0x1p23f);
-    ix &= 0x7fffffffu;
-    ix -= 23u << 23;
+    r.ix = __float_as_uint(x * 0x1p23f);
+    r.ix &= 0x7fffffffu;
+    r.ix -= 23u << 23;
   }
-  return false;
+  r.done = false;
+  return r;
 }
 
 // e_powf.c
@@ -282,8 +292,10 @@ __device__ __forceinline__ float powf_(const tables_t &tb, float x, float y)
   const uint32_t iy = __float_as_uint(y);
   if(ix - 0x00800000u >= 0x7f800000u - 0x00800000u || zeroinfnan(iy))
   {
-    float out;
-    if(powf_special(x, y, ix, iy, sign_bias, out)) return out;
+    const powf_pre_t pre = powf_special(x, y, ix, iy);
+    if(pre.done) return pre.out;
+    ix = pre.ix;
+    sign_bias = pre.sign_bias;
   }
   // log2_inline
   const uint32_t tmp = ix - OFF;
