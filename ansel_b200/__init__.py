@@ -203,6 +203,64 @@ class DitherData(C.Structure):
     _fields_ = [("dither_type", C.c_int), ("radius", C.c_float), ("range", C.c_float * 4), ("damping", C.c_float), ("levels", C.c_int)]
 
 
+LENS_MODIFY_TCA, LENS_MODIFY_VIGNETTING, LENS_MODIFY_DISTORTION, LENS_MODIFY_GEOMETRY, LENS_MODIFY_SCALE = 0x01, 0x02, 0x08, 0x10, 0x20
+LS_DIST_NONE, LS_DIST_POLY3, LS_DIST_POLY5, LS_DIST_PTLENS, LS_DIST_KNOTS = range(5)
+LS_TCA_NONE, LS_TCA_LINEAR, LS_TCA_POLY3 = range(3)
+LS_VIG_NONE, LS_VIG_PA, LS_VIG_KNOTS = range(3)
+(LENS_UNKNOWN, LENS_RECTILINEAR, LENS_FISHEYE, LENS_PANORAMIC, LENS_EQUIRECTANGULAR, LENS_FISHEYE_ORTHOGRAPHIC,
+ LENS_FISHEYE_STEREOGRAPHIC, LENS_FISHEYE_EQUISOLID, LENS_FISHEYE_THOBY) = range(9)
+LS_ENABLE_DISTORTION, LS_ENABLE_TCA, LS_ENABLE_VIGNETTING, LS_ENABLE_SCALE, LS_ENABLE_GEOMETRY = 1, 2, 4, 8, 16
+IMAGE_MONOCHROME, IMAGE_MONOCHROME_BAYER = 1 << 15, 1 << 19
+LS_MAX_CALIB, LS_MAX_KNOTS = 512, 16
+
+
+class LsCalibDist(C.Structure):
+    _fields_ = [("model", C.c_int), ("focal", C.c_float), ("terms", C.c_float * 3)]
+
+
+class LsCalibTca(C.Structure):
+    _fields_ = [("model", C.c_int), ("focal", C.c_float), ("terms", C.c_float * 6)]
+
+
+class LsCalibVig(C.Structure):
+    _fields_ = [("model", C.c_int), ("focal", C.c_float), ("aperture", C.c_float), ("distance", C.c_float), ("terms", C.c_float * 3)]
+
+
+class LsCalibRealFocal(C.Structure):
+    _fields_ = [("focal", C.c_float), ("real_focal", C.c_float)]
+
+
+class LsLens(C.Structure):
+    """b200_ls_lens_t == ls_lens_t (src/external/LensSerious/include/lensserious.h:108-129)."""
+    _fields_ = [("type", C.c_int), ("crop_factor", C.c_float), ("aspect_ratio", C.c_float), ("min_focal", C.c_float), ("max_focal", C.c_float),
+                ("center_x", C.c_float), ("center_y", C.c_float),
+                ("n_dist", C.c_int), ("dist", LsCalibDist * LS_MAX_CALIB), ("n_tca", C.c_int), ("tca", LsCalibTca * LS_MAX_CALIB),
+                ("n_vig", C.c_int), ("vig", LsCalibVig * LS_MAX_CALIB), ("n_real_focal", C.c_int), ("real_focal", LsCalibRealFocal * LS_MAX_CALIB)]
+
+
+class LensData(C.Structure):
+    """b200_lens_data_t == dt_iop_lensfun_data_t (src/iop/lens.c:392-409)."""
+    _fields_ = [("modify_flags", C.c_int), ("inverse", C.c_int), ("scale", C.c_float), ("crop", C.c_float), ("focal", C.c_float),
+                ("aperture", C.c_float), ("distance", C.c_float), ("target_geom", C.c_int), ("do_nan_checks", C.c_int),
+                ("tca_override", C.c_int), ("ls_lens", LsLens), ("ls_have", C.c_int)]
+
+
+class LensPiece(C.Structure):
+    """b200_lens_piece_t: the data block + the warp interpolator process() resolves from the user preference."""
+    _fields_ = [("data", LensData), ("interpolation", C.c_int)]
+
+
+class LensEval(C.Structure):
+    """b200_lens_eval_t == ls_eval_t (src/external/LensSerious/include/lensserious_eval.h:143-194)."""
+    _fields_ = [("norm_scale", C.c_float), ("norm_unscale", C.c_float), ("center_x", C.c_float), ("center_y", C.c_float),
+                ("vig_scale", C.c_float), ("vig_center_x", C.c_float), ("vig_center_y", C.c_float), ("scale", C.c_float),
+                ("dist_model", C.c_int), ("tca_model", C.c_int), ("vig_model", C.c_int), ("enabled", C.c_int), ("geom_from", C.c_int),
+                ("geom_to", C.c_int), ("geom_focal", C.c_float), ("reverse", C.c_int), ("dist_terms", C.c_float * 3),
+                ("tca_terms", C.c_float * 6), ("vig_terms", C.c_float * 3), ("knot_n", C.c_int),
+                ("knot_r", (C.c_float * LS_MAX_KNOTS) * 3), ("knot_c", (C.c_float * LS_MAX_KNOTS) * 3), ("knot_vn", C.c_int),
+                ("knot_vr", C.c_float * LS_MAX_KNOTS), ("knot_v", C.c_float * LS_MAX_KNOTS)]
+
+
 class B200Error(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"libb200iop error {code}: {msg}")
@@ -231,7 +289,13 @@ def lib() -> C.CDLL:
             getattr(L, f"b200_{op}_process_dev").argtypes = [C.POINTER(Piece), C.c_void_p, C.c_void_p, C.c_void_p]
             getattr(L, f"b200_{op}_tiling").argtypes = [C.POINTER(Piece), C.POINTER(Tiling)]
             getattr(L, f"b200_{op}_tiling").restype = None
-        L.b200_highlights_laplacian_dev.argtypes = [C.POINTER(Piece), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        # lens correction (piece->data: a b200_lens_piece_t from lens_piece()) and its host plan
+        L.b200_lens_process_host.argtypes = [C.POINTER(Piece), C.c_void_p, C.c_void_p]
+        L.b200_lens_process_dev.argtypes = [C.POINTER(Piece), C.c_void_p, C.c_void_p, C.c_void_p]
+        L.b200_lens_tiling.argtypes = [C.POINTER(Piece), C.POINTER(Tiling)]
+        L.b200_lens_tiling.restype = None
+        L.b200_lens_plan.argtypes = [C.POINTER(LensData), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(LensEval)]
+        L.b200_highlights_laplacian_dev.argtypes =[C.POINTER(Piece), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.b200_rawfront_process_dev.argtypes = [C.POINTER(Piece), C.POINTER(Piece), C.POINTER(Piece), C.c_void_p, C.c_void_p, C.c_void_p]
         L.b200_resampling_plan.argtypes = [C.c_int] * 5 + [C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
         L.b200_basebuffer_upload_dev.argtypes = [C.POINTER(Piece), C.c_void_p, C.c_int, C.c_int, C.c_size_t, C.c_void_p, C.c_void_p]
@@ -554,3 +618,11 @@ def dither_data(dither_type: int = DITHER_FSAUTO, levels: int = IMAGEIO_RGB | IM
     d.damping = -200.0
     d.levels = levels
     return d
+
+
+def lens_piece(data: LensData, interpolation: int = INTERPOLATION_MITCHELL) -> LensPiece:
+    """b200_lens_piece_t: a copy of the data block + the warp interpolator (the preference's default: Mitchell)"""
+    lp = LensPiece()
+    C.memmove(C.addressof(lp.data), C.addressof(data), C.sizeof(LensData))
+    lp.interpolation = interpolation
+    return lp

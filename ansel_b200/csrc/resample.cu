@@ -17,6 +17,7 @@
 #include <math.h>
 #include <string.h>
 #include <vector>
+#include "interp_taps.cuh"
 
 namespace
 {
@@ -30,20 +31,6 @@ struct axis_plan_t
 
 inline float ceil_fast(float x) { return x <= 0.f ? (float)(int)x : -((float)(int)-x) + 1.f; } // math/math.h:324-334
 inline int half_width(int interpolator) { return interpolator == B200_INTERPOLATION_BILINEAR ? 1 : 2; }
-
-// one tap weight at position t: _maketaps_bilinear :186, _maketaps_bicubic :219-228, _maketaps_mitchell :272-282
-inline float tap_weight(int interpolator, float t)
-{
-  const float a = fabsf(t);
-  if(interpolator == B200_INTERPOLATION_BILINEAR) return 1.0f - a;
-  if(interpolator == B200_INTERPOLATION_BICUBIC)
-  {
-    const float t2 = t * t, t5 = 5.0f * a;
-    return a <= 1.0f ? ((3.0f * t2 - t5) * a + 2.0f) * 0.5f : (a * (t5 - 8.0f - t2) + 4.0f) * 0.5f;
-  }
-  const float a2 = a * a, a3 = a2 * a;
-  return a <= 1.0f ? (7.0f / 6.0f) * a3 - 2.0f * a2 + (8.0f / 9.0f) : 2.0f * a2 - (7.0f / 18.0f) * a3 - (10.0f / 3.0f) * a + (16.0f / 9.0f);
-}
 // the reference generates taps four at a time: lane k starts at first + k * interval and every lane advances by
 // 4 * interval per group, so tap n sits at (((first + (n % 4) * interval) + 4 interval) + 4 interval) ...  (n / 4 times)
 inline void make_taps(int interpolator, float *taps, int num_taps, float first_tap, float interval)

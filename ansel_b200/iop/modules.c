@@ -158,6 +158,45 @@ void dt_iop_initialscale__tiling_callback(struct dt_iop_module_t *self, const dt
   b200_initialscale_tiling(&p, tiling);
 }
 
+/* lens correction's process() resolves its interpolator from the user preference (dt_interpolation_new(DT_INTERPOLATION_USERPREF_WARP),
+ * lens.c:716); the adapter carries it next to a copy of the data block.  Which images are monochrome comes with the piece
+ * (image_flags). */
+int b200_userpref_warp_interpolator = B200_INTERPOLATION_MITCHELL; /* plugins/lighttable/export/pixel_interpolator_warp, default "mitchell" */
+static int lens_view(b200_lens_piece_t *lp, b200_piece_t *p, const dt_dev_pixelpipe_iop_t *piece)
+{
+  if(!piece->data || piece->data_size < sizeof(b200_lens_data_t)) return 1;
+  memcpy(&lp->data, piece->data, sizeof(b200_lens_data_t));
+  lp->interpolation = b200_userpref_warp_interpolator;
+  p->data = lp;
+  p->data_size = sizeof(*lp);
+  return 0;
+}
+int dt_iop_lens__process(struct dt_iop_module_t *self, const dt_dev_pixelpipe_t *pipe, const dt_dev_pixelpipe_iop_t *piece, const void *const i,
+                         void *const o)
+{
+  b200_piece_t p;
+  static _Thread_local b200_lens_piece_t lp; /* 45 KB: kept off the caller's stack */
+  b200_piece_from_dt(&p, self, pipe, piece);
+  if(lens_view(&lp, &p, piece)) return 1;
+  return b200_lens_process_host(&p, i, o);
+}
+int dt_iop_lens__process_cl(struct dt_iop_module_t *self, const dt_dev_pixelpipe_t *pipe, const dt_dev_pixelpipe_iop_t *piece, cl_mem dev_in,
+                            cl_mem dev_out)
+{
+  b200_piece_t p;
+  static _Thread_local b200_lens_piece_t lp;
+  b200_piece_from_dt(&p, self, pipe, piece);
+  if(lens_view(&lp, &p, piece)) return FALSE;
+  return b200_lens_process_dev(&p, dev_in, dev_out, pipe->stream) == 0 ? TRUE : FALSE;
+}
+void dt_iop_lens__tiling_callback(struct dt_iop_module_t *self, const dt_dev_pixelpipe_t *pipe, const dt_dev_pixelpipe_iop_t *piece,
+                                  dt_develop_tiling_t *tiling)
+{
+  b200_piece_t p;
+  b200_piece_from_dt(&p, self, pipe, piece);
+  b200_lens_tiling(&p, tiling); /* reads nothing of the piece */
+}
+
 /* dither's process() reads pipe->levels next to piece->data (get_dither_parameters, dither.c:285-314): the adapter copies the
  * data block and adds it */
 static int dither_view(b200_dither_data_t *dd, b200_piece_t *p, const dt_dev_pixelpipe_t *pipe, const dt_dev_pixelpipe_iop_t *piece)

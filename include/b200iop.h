@@ -735,6 +735,146 @@ int b200_dither_process_host(const b200_piece_t *piece, const void *in, void *ou
 int b200_dither_process_dev(const b200_piece_t *piece, const void *d_in, void *d_out, void *stream);
 void b200_dither_tiling(const b200_piece_t *piece, b200_tiling_t *tiling); /* default_tiling_callback: the module declares none */
 
+/* ---- lens correction (src/iop/lens.c): distortion, TCA and vignetting through LensSerious's evaluators ------------------- */
+/* dt_lens_modify_t, lens.c:121-129 (same values) */
+enum
+{
+  B200_LENS_MODIFY_TCA = 0x01,
+  B200_LENS_MODIFY_VIGNETTING = 0x02,
+  B200_LENS_MODIFY_DISTORTION = 0x08,
+  B200_LENS_MODIFY_GEOMETRY = 0x10,
+  B200_LENS_MODIFY_SCALE = 0x20
+};
+/* ls_dist_model_t, ls_tca_model_t, ls_vig_model_t (src/external/LensSerious/include/lensserious.h:61-82, same values) */
+enum
+{
+  B200_LS_DIST_NONE = 0,
+  B200_LS_DIST_POLY3 = 1,
+  B200_LS_DIST_POLY5 = 2,
+  B200_LS_DIST_PTLENS = 3,
+  B200_LS_DIST_KNOTS = 4,
+  B200_LS_TCA_NONE = 0,
+  B200_LS_TCA_LINEAR = 1,
+  B200_LS_TCA_POLY3 = 2,
+  B200_LS_VIG_NONE = 0,
+  B200_LS_VIG_PA = 1,
+  B200_LS_VIG_KNOTS = 2
+};
+/* ls_lens_type_t (lensserious.h:94-105) == dt_lens_type_t (lens.c:131-142) */
+enum
+{
+  B200_LENS_UNKNOWN = 0,
+  B200_LENS_RECTILINEAR = 1,
+  B200_LENS_FISHEYE = 2,
+  B200_LENS_PANORAMIC = 3,
+  B200_LENS_EQUIRECTANGULAR = 4,
+  B200_LENS_FISHEYE_ORTHOGRAPHIC = 5,
+  B200_LENS_FISHEYE_STEREOGRAPHIC = 6,
+  B200_LENS_FISHEYE_EQUISOLID = 7,
+  B200_LENS_FISHEYE_THOBY = 8
+};
+/* LS_ENABLE_* (lensserious.h:131-135, same values): the axes a plan resolved */
+enum
+{
+  B200_LS_ENABLE_DISTORTION = 1 << 0,
+  B200_LS_ENABLE_TCA = 1 << 1,
+  B200_LS_ENABLE_VIGNETTING = 1 << 2,
+  B200_LS_ENABLE_SCALE = 1 << 3,
+  B200_LS_ENABLE_GEOMETRY = 1 << 4
+};
+#define B200_IMAGE_MONOCHROME (1u << 15)       /* DT_IMAGE_MONOCHROME, common/image.h:141 */
+#define B200_IMAGE_MONOCHROME_BAYER (1u << 19) /* DT_IMAGE_MONOCHROME_BAYER, common/image.h:150 */
+#define B200_LS_MAX_CALIB 512
+#define B200_LS_MAX_KNOTS 16
+/* ls_calib_*_t and ls_lens_t, lensserious.h:85-129 (identical layout: the enums are ints) */
+typedef struct b200_ls_calib_dist_t
+{
+  int model; /* B200_LS_DIST_* */
+  float focal;
+  float terms[3];
+} b200_ls_calib_dist_t;
+typedef struct b200_ls_calib_tca_t
+{
+  int model; /* B200_LS_TCA_* */
+  float focal;
+  float terms[6];
+} b200_ls_calib_tca_t;
+typedef struct b200_ls_calib_vig_t
+{
+  int model; /* B200_LS_VIG_* */
+  float focal, aperture, distance;
+  float terms[3];
+} b200_ls_calib_vig_t;
+typedef struct b200_ls_calib_real_focal_t
+{
+  float focal, real_focal;
+} b200_ls_calib_real_focal_t;
+typedef struct b200_ls_lens_t
+{
+  int type; /* B200_LENS_* */
+  float crop_factor, aspect_ratio, min_focal, max_focal, center_x, center_y;
+  int n_dist;
+  b200_ls_calib_dist_t dist[B200_LS_MAX_CALIB];
+  int n_tca;
+  b200_ls_calib_tca_t tca[B200_LS_MAX_CALIB];
+  int n_vig;
+  b200_ls_calib_vig_t vig[B200_LS_MAX_CALIB];
+  int n_real_focal;
+  b200_ls_calib_real_focal_t real_focal[B200_LS_MAX_CALIB];
+} b200_ls_lens_t;
+/* dt_iop_lensfun_data_t, lens.c:392-409 (identical layout, 45144 bytes) */
+typedef struct b200_lens_data_t
+{
+  int modify_flags; /* B200_LENS_MODIFY_* */
+  int inverse;
+  float scale, crop, focal, aperture, distance;
+  int target_geom; /* B200_LENS_* */
+  int do_nan_checks;
+  int tca_override;
+  b200_ls_lens_t ls_lens;
+  int ls_have;
+} b200_lens_data_t;
+/* what process() reads: piece->data plus the warp interpolator it resolves from the user preference
+ * (dt_interpolation_new(DT_INTERPOLATION_USERPREF_WARP), plugins/lighttable/export/pixel_interpolator_warp, default "mitchell") */
+typedef struct b200_lens_piece_t
+{
+  b200_lens_data_t data;
+  int interpolation; /* B200_INTERPOLATION_* */
+} b200_lens_piece_t;
+/* ls_eval_t, src/external/LensSerious/include/lensserious_eval.h:143-194 (identical layout, 632 bytes): the lens resolved at one
+ * shooting configuration, the block every output pixel evaluates */
+typedef struct b200_lens_eval_t
+{
+  float norm_scale, norm_unscale, center_x, center_y;
+  float vig_scale, vig_center_x, vig_center_y;
+  float scale;
+  int dist_model, tca_model, vig_model, enabled, geom_from, geom_to;
+  float geom_focal;
+  int reverse;
+  float dist_terms[3], tca_terms[6], vig_terms[3];
+  int knot_n;
+  float knot_r[3][B200_LS_MAX_KNOTS], knot_c[3][B200_LS_MAX_KNOTS];
+  int knot_vn;
+  float knot_vr[B200_LS_MAX_KNOTS], knot_v[B200_LS_MAX_KNOTS];
+} b200_lens_eval_t;
+/* The host plan of process(): get_modifier (lens.c:620-653) = ls_modifier_init + ls_eval_from_modifier
+ * (src/external/LensSerious/src/lensserious.c:36-407, 707-777) over a width x height frame, with TCA left out of the request
+ * for monochrome images (lens.c:698-699).  *modflags receives the DT_LENS_MODIFY_* axes resolved, *eval the block.  Returns
+ * B200_OK, or B200_ERR_ARG on NULL pointers.  Host only: needs no device. */
+int b200_lens_plan(const b200_lens_data_t *d, int width, int height, int monochrome, int *modflags, b200_lens_eval_t *eval);
+/* process() :680-923 on roi_in -> roi_out RGBA float (piece->channels == 4), piece->data a b200_lens_piece_t: both directions
+ * (data->inverse), distortion (poly3, poly5, ptlens), TCA (linear, poly3), the scale, pa vignetting folded into the resampling
+ * (at each channel's source position when correcting, at the destination when reversing), do_nan_checks, monochrome images
+ * (piece->image_flags & (B200_IMAGE_MONOCHROME | B200_IMAGE_MONOCHROME_BAYER)), bilinear / bicubic / Mitchell sampling with the
+ * reference's mirrored border; lane 3 is resampled from the green source position under B200_DISPLAY_MASK and left as the
+ * caller's buffer holds it otherwise.  No geometry resolved: the frame is copied (and vignetted); no lens or crop <= 0: copied.
+ * The plan is cached per data block and frame size.  B200_ERR_UNSUPPORTED, output untouched: a projection change (the plan
+ * resolves LS_ENABLE_GEOMETRY: its tanf/asinf are not restated), knot tables, roi_in under 3 x 3 px when resampling (the
+ * reference's mirrored taps leave the buffer), and a copy between ROIs of different sizes. */
+int b200_lens_process_host(const b200_piece_t *piece, const void *in, void *out);
+int b200_lens_process_dev(const b200_piece_t *piece, const void *d_in, void *d_out, void *stream);
+void b200_lens_tiling(const b200_piece_t *piece, b200_tiling_t *tiling); /* tiling_callback :1065-1098: factor 2, overlap 4 */
+
 /* ---- basebuffer (src/iop/basebuffer.c): the pipe's first node, sensor buffer -> first cacheline ------------------------- */
 /* process() :119-160 copies the crop roi_out out of the full-size buffer the mipmap cache holds (host memory, pipe->iwidth x
  * pipe->iheight samples of dsc_in.bpp bytes) into the module's output.  On the device that copy IS the upload: one strided
