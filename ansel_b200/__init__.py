@@ -21,6 +21,7 @@ PIPE_NONE, PIPE_EXPORT, PIPE_FULL, PIPE_PREVIEW, PIPE_THUMBNAIL = range(5)
 
 DEMOSAIC_PPG, DEMOSAIC_AMAZE, DEMOSAIC_VNG4, DEMOSAIC_RCD, DEMOSAIC_LMMSE = 0, 1, 2, 5, 6
 DEMOSAIC_MARKESTEIJN_3_VNG = 3074  # DT_IOP_DEMOSAIC_MARKEST3_VNG: X-Trans Markesteijn 3-pass + VNG, iop/demosaic.c:138
+DEMOSAIC_FDC = 1028  # DT_IOP_DEMOSAIC_FDC: X-Trans frequency-domain chroma, iop/demosaic.c:137 (piece->data: a DemosaicPiece)
 DT_IMAGE_4BAYER = 1 << 14  # b200_piece_t.image_flags of a four-colour Bayer sensor (CYGM, RGBE), common/image.h
 GREEN_EQ_NO, GREEN_EQ_LOCAL, GREEN_EQ_FULL, GREEN_EQ_BOTH = 0, 1, 2, 3  # dt_iop_demosaic_greeneq_t, iop/demosaic.c:146-149
 
@@ -51,6 +52,11 @@ class DemosaicData(C.Structure):
     _fields_ = [("green_eq", C.c_uint32), ("color_smoothing", C.c_uint32), ("demosaicing_method", C.c_uint32),
                 ("lmmse_refine", C.c_uint32), ("median_thrs", C.c_float), ("CAM_to_RGB", (C.c_double * 4) * 3),
                 ("dual_thrs", C.c_float)]
+
+
+class DemosaicPiece(C.Structure):
+    """b200_demosaic_piece_t: the data block + the user's FDC crossover ISO (plugins/darkroom/demosaic/fdc_xover_iso, default 1600)."""
+    _fields_ = [("data", DemosaicData), ("fdc_xover_iso", C.c_int)]
 
 
 LUT_SAMPLES = 0x10000

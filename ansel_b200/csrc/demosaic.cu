@@ -21,6 +21,7 @@ int downsample_xtrans_demosaic_dev(const float *d_in, float *d_out, int width, i
 int ppg_demosaic_dev(const float *d_in, float *d_out, int width, int height, uint32_t filters, float median_thrs, cudaStream_t s);
 int lmmse_demosaic_dev(const float *d_in, float *d_out, int width, int height, uint32_t filters, int mode, const float processed_maximum[3], cudaStream_t stream);
 int markesteijn_demosaic_dev(const float *d_in, float *d_out, int width, int height, int x0, int y0, const uint8_t xtrans[6][6], int passes, cudaStream_t stream);
+int fdc_demosaic_dev(const float *d_in, float *d_out, int width, int height, int x0, int y0, const uint8_t xtrans[6][6], int pure, cudaStream_t stream);
 int demosaic_green_eq_dev(const float *d_in, float *d_tmp0, float *d_tmp1, double *d_partial, int width, int height, uint32_t dsc_filters, int x, int y,
                           unsigned green_eq, float threshold, const float **d_result, cudaStream_t s);
 int demosaic_green_eq_partial_doubles();
@@ -33,7 +34,10 @@ using namespace b200;
 #define MARKEST3_VNG (DEMOSAIC_DUAL | 1026u) /* DT_IOP_DEMOSAIC_MARKEST3_VNG, iop/demosaic.c:138 */
 
 // methods that, like the reference, leave (part of) the alpha lane as they find it
-static bool keeps_alpha(uint32_t m) { return m == B200_DEMOSAIC_PPG || m == 3u || m == 4u || m == 1024u || m == 1025u || m == 1026u || m == MARKEST3_VNG; }
+static bool keeps_alpha(uint32_t m)
+{
+  return m == B200_DEMOSAIC_PPG || m == 3u || m == 4u || m == 1024u || m == 1025u || m == 1026u || m == B200_DEMOSAIC_FDC || m == MARKEST3_VNG;
+}
 
 static int check_piece(const b200_piece_t *piece, const void *in, void *out)
 {
@@ -91,10 +95,23 @@ extern "C" int b200_demosaic_process_dev(const b200_piece_t *piece, const void *
     // (DT_IOP_DEMOSAIC_MARKESTEIJN_3 = 1026, and MARKEST3_VNG = 3074, which blends in VNG after it, :1243-1247); VNG is what every
     // X-Trans method below them resolves to (DT_IOP_DEMOSAIC_VNG = 1024)
     const uint32_t m = d->demosaicing_method;
-    if(m != 1024u && m != 1025u && m != 1026u && m != MARKEST3_VNG)
-      return fail(B200_ERR_UNSUPPORTED, "demosaic: X-Trans method %u is not built (VNG, Markesteijn and Markesteijn 3-pass + VNG are; FDC is not)", m);
+    if(m != 1024u && m != 1025u && m != 1026u && m != MARKEST3_VNG && m != B200_DEMOSAIC_FDC)
+      return fail(B200_ERR_UNSUPPORTED, "demosaic: X-Trans method %u is not built (VNG, Markesteijn, Markesteijn 3-pass + VNG and FDC are)", m);
+    if(m == B200_DEMOSAIC_FDC && piece->data_size < sizeof(b200_demosaic_piece_t))
+      return fail(B200_ERR_UNSUPPORTED, "demosaic: FDC is not built for a bare b200_demosaic_data_t: it needs fdc_xover_iso, the user's crossover ISO "
+                                        "(pass a b200_demosaic_piece_t)");
     if(piece->roi_out.width != piece->roi_in.width || piece->roi_out.height != piece->roi_in.height)
       return fail(B200_ERR_UNSUPPORTED, "demosaic: roi_out != roi_in (downsampling paths are not built)");
+    if(m == B200_DEMOSAIC_FDC)
+    { // demosaic.c:1124-1125, then colour smoothing (:1249); markesteijn.c:1137-1139: int iso = exif_iso, pure FDC above the crossover
+      const int iso = (int)piece->exif_iso, pure = iso > ((const b200_demosaic_piece_t *)piece->data)->fdc_xover_iso;
+      rc = fdc_demosaic_dev((const float *)d_in, (float *)d_out, piece->roi_in.width, piece->roi_in.height, piece->roi_in.x, piece->roi_in.y, piece->xtrans,
+                            pure, (cudaStream_t)stream);
+      if(rc) return rc;
+      if(d->color_smoothing)
+        rc = demosaic_color_smoothing_dev((float *)d_out, piece->roi_out.width, piece->roi_out.height, (int)d->color_smoothing, (cudaStream_t)stream);
+      return rc;
+    }
     if(m == 1025u || m == 1026u || m == MARKEST3_VNG)
     {
       rc = markesteijn_demosaic_dev((const float *)d_in, (float *)d_out, piece->roi_in.width, piece->roi_in.height, piece->roi_in.x, piece->roi_in.y,

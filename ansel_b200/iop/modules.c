@@ -35,7 +35,43 @@
     b200_##op##_tiling(&p, tiling);                                                                       \
   }
 
-ADAPT(demosaic) /* src/iop/demosaic.c:1043 (process), rcd.c:568 (process_rcd_cl), :1916 (tiling_callback) */
+/* demosaic: src/iop/demosaic.c:1043 (process), rcd.c:568 (process_rcd_cl), :1916 (tiling_callback).  FDC's process() reads the user's
+ * crossover ISO (markesteijn.c:1137); the adapter carries it next to a copy of the data block. */
+int b200_userpref_fdc_xover_iso = 1600; /* plugins/darkroom/demosaic/fdc_xover_iso, data/anselconfig.xml.in:1814 */
+static int demosaic_view(b200_demosaic_piece_t *dp, b200_piece_t *p, const dt_dev_pixelpipe_iop_t *piece)
+{
+  if(!piece->data || piece->data_size < sizeof(b200_demosaic_data_t)) return 1;
+  memcpy(&dp->data, piece->data, sizeof(b200_demosaic_data_t));
+  dp->fdc_xover_iso = b200_userpref_fdc_xover_iso;
+  p->data = dp;
+  p->data_size = sizeof(*dp);
+  return 0;
+}
+int dt_iop_demosaic__process(struct dt_iop_module_t *self, const dt_dev_pixelpipe_t *pipe, const dt_dev_pixelpipe_iop_t *piece, const void *const i,
+                             void *const o)
+{
+  b200_piece_t p;
+  b200_demosaic_piece_t dp;
+  b200_piece_from_dt(&p, self, pipe, piece);
+  if(demosaic_view(&dp, &p, piece)) return 1;
+  return b200_demosaic_process_host(&p, i, o);
+}
+int dt_iop_demosaic__process_cl(struct dt_iop_module_t *self, const dt_dev_pixelpipe_t *pipe, const dt_dev_pixelpipe_iop_t *piece, cl_mem dev_in,
+                                cl_mem dev_out)
+{
+  b200_piece_t p;
+  b200_demosaic_piece_t dp;
+  b200_piece_from_dt(&p, self, pipe, piece);
+  if(demosaic_view(&dp, &p, piece)) return FALSE;
+  return b200_demosaic_process_dev(&p, dev_in, dev_out, pipe->stream) == 0 ? TRUE : FALSE;
+}
+void dt_iop_demosaic__tiling_callback(struct dt_iop_module_t *self, const dt_dev_pixelpipe_t *pipe, const dt_dev_pixelpipe_iop_t *piece,
+                                      dt_develop_tiling_t *tiling)
+{
+  b200_piece_t p;
+  b200_piece_from_dt(&p, self, pipe, piece);
+  b200_demosaic_tiling(&p, tiling);
+}
 ADAPT(colorin)  /* src/iop/colorin.c:711, :590-681 (process_cl) */
 ADAPT(colorout) /* src/iop/colorout.c:373, :288-371 (process_cl) */
 

@@ -168,6 +168,15 @@ typedef struct b200_demosaic_data_t
 } b200_demosaic_data_t;
 
 #define B200_DEMOSAIC_DUAL 2048 /* DEMOSAIC_DUAL, iop/demosaic.c:109: or-ed into the method */
+#define B200_DEMOSAIC_FDC 1028  /* DT_IOP_DEMOSAIC_FDC, iop/demosaic.c:137: frequency-domain chroma, X-Trans */
+/* what process() reads for FDC: piece->data plus the user's crossover ISO (dt_conf plugins/darkroom/demosaic/fdc_xover_iso, default 1600,
+ * markesteijn.c:1137): above it (int(piece->exif_iso) > fdc_xover_iso) chroma is pure FDC, at and below it hybrid.  Recognised by
+ * piece->data_size; a bare b200_demosaic_data_t cannot name the crossover, so FDC refuses it. */
+typedef struct b200_demosaic_piece_t
+{
+  b200_demosaic_data_t data;
+  int fdc_xover_iso;
+} b200_demosaic_piece_t;
 /* process(), iop/demosaic.c:1043-1253: in = 1-channel float mosaic roi_in, out = RGBA float roi_out.  Built for Bayer
  * sensors: RCD (iop/demosaic/rcd.c), AMaZE (amaze.cc), LMMSE (lmmse.c; data->lmmse_refine; every tile from zeroed planes, where the
  * reference carries them from tile to tile: DESIGN.md row f12), PPG with its optional pre-median (ppg.c, basic.c:136-186;
@@ -176,13 +185,16 @@ typedef struct b200_demosaic_data_t
  * (data->green_eq) and median colour smoothing behind (data->color_smoothing); the two passthrough methods (3 monochrome,
  * 4 photosite colour; passthrough.c) for any sensor; for X-Trans sensors (filters == 9, piece->xtrans) Markesteijn with one pass
  * (method 1025, the default of X-Trans frames; markesteijn.c:47-521) or three (method 1026), Markesteijn 3-pass + VNG (method 3074:
- * the dual blend with X-Trans VNG, data->dual_thrs, piece->wb_coeffs; lane 3 is kept as the caller's buffer holds it) and VNG
- * (method 1024, the X-Trans branch of vng.c); on four-colour Bayer sensors (piece->image_flags & (1 << 14), DT_IMAGE_4BAYER: CYGM,
+ * the dual blend with X-Trans VNG, data->dual_thrs, piece->wb_coeffs; lane 3 is kept as the caller's buffer holds it), VNG
+ * (method 1024, the X-Trans branch of vng.c) and frequency-domain chroma (method 1028, B200_DEMOSAIC_FDC, markesteijn.c:525-1639:
+ * piece->data a b200_demosaic_piece_t; every tile from a zeroed scratch, where the reference carries part of it from tile to tile;
+ * lane 3 is kept as the caller's buffer holds it; frames of 14 px or less a side are refused); on four-colour Bayer sensors (piece->image_flags & (1 << 14), DT_IMAGE_4BAYER: CYGM,
  * RGBE) every full-size method runs VNG with the sensor's word and then data->CAM_to_RGB (demosaic.c:1173-1183; no green
  * equilibration; lane 3 is the fourth camera colour), followed by the dual blend for RCD|DUAL and AMaZE|DUAL; the
  * half-size downsample (method 7, iop/demosaic.c:480-532 Bayer, :543-666 X-Trans; roi_out =
  * (roi_in + 1) / 2; four-colour Bayer sensors through data->CAM_to_RGB) and its guided-Laplacian post-filter (:681-926;
- * data->color_smoothing iterations).  FDC and the GUI's mask display return B200_ERR_UNSUPPORTED. */
+ * data->color_smoothing iterations).  FDC with a bare b200_demosaic_data_t, FDC on other sensors and the GUI's mask display return
+ * B200_ERR_UNSUPPORTED. */
 int b200_demosaic_process_host(const b200_piece_t *piece, const void *in, void *out);
 /* process_cl() slot, iop/demosaic/rcd.c:568-850: device pointers, `stream` is a cudaStream_t (NULL = default) */
 int b200_demosaic_process_dev(const b200_piece_t *piece, const void *d_in, void *d_out, void *stream);
