@@ -267,6 +267,27 @@ class LensEval(C.Structure):
                 ("knot_vr", C.c_float * LS_MAX_KNOTS), ("knot_v", C.c_float * LS_MAX_KNOTS)]
 
 
+COLORBALANCE_SATURATION_JZAZBZ, COLORBALANCE_SATURATION_DTUCS = 0, 1
+COLORBALANCE_LUT_ELEM = 360
+
+
+class ColorbalancergbData(C.Structure):
+    """b200_colorbalancergb_data_t == dt_iop_colorbalancergb_data_t up to work_profile (src/iop/colorbalancergb.c:165-189), 232 bytes."""
+    _fields_ = [("global_", C.c_float * 4), ("shadows", C.c_float * 4), ("highlights", C.c_float * 4), ("midtones", C.c_float * 4),
+                ("midtones_Y", C.c_float), ("chroma_global", C.c_float), ("chroma", C.c_float * 4), ("vibrance", C.c_float),
+                ("contrast", C.c_float), ("saturation_global", C.c_float), ("saturation", C.c_float * 4), ("brilliance_global", C.c_float),
+                ("brilliance", C.c_float * 4), ("hue_angle", C.c_float), ("shadows_weight", C.c_float), ("highlights_weight", C.c_float),
+                ("midtones_weight", C.c_float), ("mask_grey_fulcrum", C.c_float), ("white_fulcrum", C.c_float), ("grey_fulcrum", C.c_float),
+                ("max_chroma", C.c_float), ("checker_color_1", C.c_float * 4), ("checker_color_2", C.c_float * 4),
+                ("saturation_formula", C.c_int), ("checker_size", C.c_size_t), ("mask_preview_black_and_white", C.c_int),
+                ("mask_display", C.c_int), ("mask_type", C.c_int), ("lut_inited", C.c_int)]
+
+
+class ColorbalancergbPiece(C.Structure):
+    """b200_colorbalancergb_piece_t: the data block, the work profile's matrices and the 360 floats of the gamut LUT."""
+    _fields_ = [("data", ColorbalancergbData), ("work_profile", ProfileMatrices), ("gamut_LUT", C.c_float * COLORBALANCE_LUT_ELEM)]
+
+
 class B200Error(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"libb200iop error {code}: {msg}")
@@ -301,6 +322,11 @@ def lib() -> C.CDLL:
         L.b200_lens_tiling.argtypes = [C.POINTER(Piece), C.POINTER(Tiling)]
         L.b200_lens_tiling.restype = None
         L.b200_lens_plan.argtypes = [C.POINTER(LensData), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(LensEval)]
+        # colour balance rgb (piece->data: a b200_colorbalancergb_piece_t from colorbalancergb_piece())
+        L.b200_colorbalancergb_process_host.argtypes = [C.POINTER(Piece), C.c_void_p, C.c_void_p]
+        L.b200_colorbalancergb_process_dev.argtypes = [C.POINTER(Piece), C.c_void_p, C.c_void_p, C.c_void_p]
+        L.b200_colorbalancergb_tiling.argtypes = [C.POINTER(Piece), C.POINTER(Tiling)]
+        L.b200_colorbalancergb_tiling.restype = None
         L.b200_highlights_laplacian_dev.argtypes =[C.POINTER(Piece), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.b200_rawfront_process_dev.argtypes = [C.POINTER(Piece), C.POINTER(Piece), C.POINTER(Piece), C.c_void_p, C.c_void_p, C.c_void_p]
         L.b200_resampling_plan.argtypes = [C.c_int] * 5 + [C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
@@ -632,3 +658,19 @@ def lens_piece(data: LensData, interpolation: int = INTERPOLATION_MITCHELL) -> L
     C.memmove(C.addressof(lp.data), C.addressof(data), C.sizeof(LensData))
     lp.interpolation = interpolation
     return lp
+
+
+def colorbalancergb_piece(data_blob, work, lut) -> ColorbalancergbPiece:
+    """data_blob: the 232 bytes of dt_iop_colorbalancergb_data_t commit_params() leaves (or a ColorbalancergbData); work: (matrix_in,
+    matrix_out) 3x3 arrays of the pipe's work profile; lut: the 360 floats behind data->gamut_LUT."""
+    import numpy as np
+    assert C.sizeof(ColorbalancergbData) == 232
+    cp = ColorbalancergbPiece()
+    blob = bytes(data_blob) if isinstance(data_blob, ColorbalancergbData) else np.ascontiguousarray(data_blob, np.uint8).tobytes()
+    assert len(blob) == C.sizeof(ColorbalancergbData)
+    C.memmove(C.addressof(cp.data), blob, len(blob))
+    cp.work_profile = profile_matrices(work[0], work[1])
+    lut = np.ascontiguousarray(lut, np.float32)
+    assert lut.shape == (COLORBALANCE_LUT_ELEM,)
+    C.memmove(C.addressof(cp.gamut_LUT), lut.ctypes.data, lut.nbytes)
+    return cp

@@ -62,7 +62,7 @@ class PipeNode(C.Structure):
 _mod = None
 ADAPTED_OPS = ("demosaic", "colorin", "colorout", "denoiseprofile", "filmicrgb", "bilat", "diffuse", "nlmeans",
                "rawprepare", "temperature", "highlights", "exposure", "gamma", "finalscale", "channelmixerrgb", "initialscale", "flip",
-               "dither", "lens")
+               "dither", "lens", "colorbalancergb")
 
 
 def modlib() -> C.CDLL:

@@ -129,6 +129,60 @@ void dt_iop_channelmixerrgb__tiling_callback(struct dt_iop_module_t *self, const
   b200_channelmixerrgb_tiling(&p, tiling);
 }
 
+/* colour balance rgb reads the pipe's current work profile next to piece->data (colorbalancergb.c:590-591) and the gamut LUT behind
+ * data->gamut_LUT, which commit_params() builds and the library reads as given.  piece->data_size is the hashed prefix (init_pipe
+ * :1365); the runtime pointers follow it in the reference's struct. */
+typedef struct cbrgb_ref_data_t
+{
+  b200_colorbalancergb_data_t prefix;
+  const void *work_profile;
+  const float *gamut_LUT;
+  const float *chroma_LUT;
+} cbrgb_ref_data_t;
+/* 1: not a colour balance rgb piece; -1: no work profile (process() :592 returns without writing) */
+static int colorbalancergb_view(b200_colorbalancergb_piece_t *cp, b200_piece_t *p, const dt_dev_pixelpipe_t *pipe, const dt_dev_pixelpipe_iop_t *piece)
+{
+  if(!piece->data || piece->data_size < sizeof(b200_colorbalancergb_data_t)) return 1;
+  const cbrgb_ref_data_t *d = (const cbrgb_ref_data_t *)piece->data;
+  if(!d->gamut_LUT) return 1;
+  const dt_iop_order_iccprofile_info_t *const work = dt_ioppr_get_pipe_work_profile_info(pipe); /* = dt_ioppr_get_pipe_current_profile_info(self, pipe) */
+  if(!work) return -1;
+  memcpy(&cp->data, &d->prefix, sizeof(cp->data));
+  memcpy(cp->work_profile.matrix_in, work->matrix_in, sizeof(work->matrix_in));
+  memcpy(cp->work_profile.matrix_out, work->matrix_out, sizeof(work->matrix_out));
+  memcpy(cp->gamut_LUT, d->gamut_LUT, sizeof(cp->gamut_LUT));
+  p->data = cp;
+  p->data_size = sizeof(*cp);
+  return 0;
+}
+int dt_iop_colorbalancergb__process(struct dt_iop_module_t *self, const dt_dev_pixelpipe_t *pipe, const dt_dev_pixelpipe_iop_t *piece,
+                                    const void *const i, void *const o)
+{
+  b200_piece_t p;
+  b200_colorbalancergb_piece_t cp;
+  b200_piece_from_dt(&p, self, pipe, piece);
+  const int v = colorbalancergb_view(&cp, &p, pipe, piece);
+  if(v) return v < 0 ? 0 : 1;
+  return b200_colorbalancergb_process_host(&p, i, o);
+}
+int dt_iop_colorbalancergb__process_cl(struct dt_iop_module_t *self, const dt_dev_pixelpipe_t *pipe, const dt_dev_pixelpipe_iop_t *piece,
+                                       cl_mem dev_in, cl_mem dev_out)
+{
+  b200_piece_t p;
+  b200_colorbalancergb_piece_t cp;
+  b200_piece_from_dt(&p, self, pipe, piece);
+  const int v = colorbalancergb_view(&cp, &p, pipe, piece);
+  if(v) return v < 0 ? TRUE : FALSE; /* process_cl :946-948 returns its (non-zero) default error code there: not a failure */
+  return b200_colorbalancergb_process_dev(&p, dev_in, dev_out, pipe->stream) == 0 ? TRUE : FALSE;
+}
+void dt_iop_colorbalancergb__tiling_callback(struct dt_iop_module_t *self, const dt_dev_pixelpipe_t *pipe,
+                                             const dt_dev_pixelpipe_iop_t *piece, dt_develop_tiling_t *tiling)
+{
+  b200_piece_t p;
+  b200_piece_from_dt(&p, self, pipe, piece);
+  b200_colorbalancergb_tiling(&p, tiling);
+}
+
 /* finalscale's data block is one dummy int (finalscale.c:46-51); its process() resolves the interpolator from the user
  * preference: dt_interpolation_new(DT_INTERPOLATION_USERPREF) (develop/imageop_math.c:150).  In the reference tree the
  * adapter passes that interpolator's id; standing alone, dt_surface.h keeps the preference in a variable. */

@@ -669,6 +669,52 @@ int b200_channelmixerrgb_process_host(const b200_piece_t *piece, const void *in,
 int b200_channelmixerrgb_process_dev(const b200_piece_t *piece, const void *d_in, void *d_out, void *stream);
 void b200_channelmixerrgb_tiling(const b200_piece_t *piece, b200_tiling_t *tiling);
 
+/* ---- colour balance rgb (src/iop/colorbalancergb.c): grading, saturation and gamut mapping --------------------------------- */
+enum
+{
+  B200_COLORBALANCE_SATURATION_JZAZBZ = 0, /* dt_iop_colorbalancrgb_saturation_t, colorbalancergb.c:82-86 (same values) */
+  B200_COLORBALANCE_SATURATION_DTUCS = 1
+};
+#define B200_COLORBALANCE_LUT_ELEM 360 /* LUT_ELEM, colorbalancergb.c:70: the gamut LUT, one entry per degree of hue */
+/* dt_iop_colorbalancergb_data_t, colorbalancergb.c:165-192, up to work_profile: the prefix init_pipe hashes (:1365), 232 bytes,
+ * identical layout */
+typedef struct b200_colorbalancergb_data_t
+{
+  float global[4], shadows[4], highlights[4], midtones[4];
+  float midtones_Y;
+  float chroma_global, chroma[4], vibrance, contrast;
+  float saturation_global, saturation[4];
+  float brilliance_global, brilliance[4];
+  float hue_angle;
+  float shadows_weight, highlights_weight, midtones_weight, mask_grey_fulcrum;
+  float white_fulcrum, grey_fulcrum;
+  float max_chroma;
+  float checker_color_1[4], checker_color_2[4];
+  int saturation_formula; /* B200_COLORBALANCE_SATURATION_*; any other value takes the darktable UCS branch, as process() does */
+  size_t checker_size;
+  int mask_preview_black_and_white;
+  int mask_display; /* set by commit_params :1130 on the darkroom's FULL pipe only */
+  int mask_type;
+  int lut_inited;
+} b200_colorbalancergb_data_t;
+/* what process() reads: piece->data, the matrices of the pipe's current work profile (dt_ioppr_get_pipe_current_profile_info,
+ * :590-591) and the 360 floats behind data->gamut_LUT, as commit_params() :1214-1352 left them */
+typedef struct b200_colorbalancergb_piece_t
+{
+  b200_colorbalancergb_data_t data;
+  b200_profile_matrices_t work_profile;
+  float gamut_LUT[B200_COLORBALANCE_LUT_ELEM];
+} b200_colorbalancergb_piece_t;
+/* process() :585-927 on roi_out RGBA float (piece->data a b200_colorbalancergb_piece_t): the Yrg chroma and hue rotation, the
+ * four-way grading in Filmlight RGB with the opacity masks, the luminance power and contrast, then the perceptual saturation and
+ * brilliance with gamut mapping through the LUT in JzAzBz or darktable UCS (data.saturation_formula); lane 3 is the input's.
+ * The LUT is read as given: commit_params() builds it, the library does not.  B200_ERR_UNSUPPORTED, output untouched: the mask
+ * display (data.mask_display, a darkroom preview whose checkerboard is sized by the GUI's DPI).  A pipe without a work profile
+ * never reaches this call: process() :592 returns without writing, and so does the module adapter. */
+int b200_colorbalancergb_process_host(const b200_piece_t *piece, const void *in, void *out);
+int b200_colorbalancergb_process_dev(const b200_piece_t *piece, const void *d_in, void *d_out, void *stream);
+void b200_colorbalancergb_tiling(const b200_piece_t *piece, b200_tiling_t *tiling); /* default_tiling_callback: the module declares none */
+
 /* ---- finalscale (src/iop/finalscale.c): the export's final resampling ------------------------------------------- */
 /* enum dt_interpolation_type, src/pixel/interpolation.h:38-44 (same values) */
 enum
